@@ -50,6 +50,7 @@ struct GemmParams {
   int ldo;
   int n_valid;             // columns >= n_valid are not stored
   int out_f32;             // store fp32 instead of fp16 (small bias-table GEMMs)
+  int gelu;                // AP_GEMM_GELU: out = gelu_erf(acc + bias) (never with a residual)
   // TMA epilogue (per-warp 32-row x 32-column boxes staged in 64B-swizzled shared memory)
   int tma_epi;             // 1: outputs leave through TMA stores, the residual arrives through TMA loads
   int sub_w, sub_h, sub_n; // conv modes: geometry of a warp's 32-row sub-box
@@ -94,24 +95,6 @@ struct GemmCfg {
   static_assert(STAGES >= 2, "need at least a double-buffered operand ring");
   static_assert(B_BYTES % 1024 == 0, "B stage must keep 1024B alignment");
 };
-
-// erf-GELU with ONE MUFU op: erfc(z) = 2^-q(z), q(z) = z * P6(z) fitted to -log2(erfc z) on [0, 4.3] (max relative error of
-// erfc 4.2e-5, |error of GELU| <= 1.1e-6: an order of magnitude below the fp16 resolution of the output). With
-// z = |x| / sqrt2 clamped to 4.3 (erfc(4.3) = 1.2e-9):  gelu(x) = max(x, 0) - 0.5 |x| erfc(z).
-// The previous Abramowitz-Stegun 7.1.26 form needed rcp + ex2; at K = 320 the GEGLU epilogue (16 K outputs per tile and
-// CTA) kept the 16-per-clock MUFU pipe busy for 2048 clocks against 2560 clocks of MMA.
-__device__ __forceinline__ float gelu_erf(float x) {
-  const float z = fminf(fabsf(x) * 0.70710678118654752f, 4.3f);
-  float q = fmaf(1.686094986e-05f, z, -4.376256625e-04f);
-  q = fmaf(q, z, 4.960034474e-03f);
-  q = fmaf(q, z, -3.321249048e-02f);
-  q = fmaf(q, z, 1.515097036e-01f);
-  q = fmaf(q, z, 9.176268788e-01f);
-  q = fmaf(q, z, 1.627959694e+00f);
-  float e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-q * z));
-  return fmaxf(x, 0.f) - z * 0.70710678118654752f * e;
-}
 
 
 template <int BN, int EPI>
@@ -377,6 +360,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CU
             v[4 * j + 0] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
           }
         }
+        if (p.gelu) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
+        }
         if (has_res) {
           mbar_wait_quiet(rbar, rphase);
           rphase ^= 1;
@@ -501,6 +488,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CU
           const float4 b = __ldg(b4 + j);
           v[4 * j + 0] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
         }
+      }
+      if (p.gelu) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
       }
       if (!row_ok) return;
       const bool vec_ok = (ncol + 32 <= p.n_valid) && ((p.ldo & 7) == 0);
@@ -728,6 +719,9 @@ extern "C" int ap_gemm_f16(const void* a, long long lda, int K1, const void* a2,
   p.n_valid = n_valid > 0 ? n_valid : nout;
   p.out_f32 = (flags & AP_GEMM_OUT_F32) ? 1 : 0;
   AP_REQUIRE(!(p.out_f32 && epi == EPI_GEGLU), "gemm: fp32 output is not available with GEGLU");
+  p.gelu = (flags & AP_GEMM_GELU) ? 1 : 0;
+  AP_REQUIRE(!p.gelu || (epi == EPI_LINEAR && residual == nullptr && !(ext && ext->ln_rstd)),
+             "gemm: GELU epilogue is not available with GEGLU, a residual or LayerNorm folding");
 
   CUtensorMap tmA1, tmA2, tmB;
   {

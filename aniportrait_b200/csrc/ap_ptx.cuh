@@ -13,6 +13,25 @@ namespace ap {
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// erf-GELU with ONE MUFU op: erfc(z) = 2^-q(z), q(z) = z * P6(z) fitted to -log2(erfc z) on [0, 4.3] (max relative error of
+// erfc 4.2e-5, |error of GELU| <= 1.1e-6: an order of magnitude below the fp16 resolution of the output). With
+// z = |x| / sqrt2 clamped to 4.3 (erfc(4.3) = 1.2e-9):  gelu(x) = max(x, 0) - 0.5 |x| erfc(z).
+// The previous Abramowitz-Stegun 7.1.26 form needed rcp + ex2; at K = 320 the GEGLU epilogue (16 K outputs per tile and
+// CTA) kept the 16-per-clock MUFU pipe busy for 2048 clocks against 2560 clocks of MMA. Shared by the GEGLU and GELU GEMM
+// epilogues, the BatchNorm apply and the wav2vec2 positional convolution.
+__device__ __forceinline__ float gelu_erf(float x) {
+  const float z = fminf(fabsf(x) * 0.70710678118654752f, 4.3f);
+  float q = fmaf(1.686094986e-05f, z, -4.376256625e-04f);
+  q = fmaf(q, z, 4.960034474e-03f);
+  q = fmaf(q, z, -3.321249048e-02f);
+  q = fmaf(q, z, 1.515097036e-01f);
+  q = fmaf(q, z, 9.176268788e-01f);
+  q = fmaf(q, z, 1.627959694e+00f);
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-q * z));
+  return fmaxf(x, 0.f) - z * 0.70710678118654752f * e;
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

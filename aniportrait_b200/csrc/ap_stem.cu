@@ -1,4 +1,4 @@
-// PoseGuider building blocks that are not GEMM-shaped: train-mode BatchNorm (+ReLU) over channels-last activations and the
+// PoseGuider building blocks that are not GEMM-shaped: train-mode BatchNorm (+ReLU / GELU) over channels-last activations and the
 // small-channel (3..64) k3/k4 convolutions of its stem.
 //
 // Replaces nn.BatchNorm2d in TRAIN mode (the reference never calls .eval() on the PoseGuider: batch statistics over the
@@ -18,7 +18,9 @@ namespace ap {
 // BatchNorm, batch statistics. x: [rows, C] fp16 (rows = frames*H*W), C % 8 == 0.
 // Stage 1: block = (C/8) * k threads, each thread owns 8 channels and strides over the block's rows; per-channel
 //          {sum, sumsq} partials per block.   Stage 2: one thread per channel adds the partials in double, in block order,
-//          and emits the affine pair a = gamma * rstd, b = beta - mean * a.   Stage 3: y = relu(a x + b).
+//          and emits the affine pair a = gamma * rstd, b = beta - mean * a.   Stage 3: y = act(a x + b).
+// For one clip, wav2vec2's GroupNorm(512 groups, 512 channels) over time is exactly this per-channel batch normalisation
+// over the [T0, 512] rows of its first convolution (act = GELU).
 // ---------------------------------------------------------------------------------------------------------
 __global__ void bn_stats_kernel(const __half* __restrict__ x, long long rows, int C, int rows_per_block,
                                 float2* __restrict__ partials) {
@@ -83,7 +85,7 @@ __global__ void bn_finalize_kernel(const float2* __restrict__ partials, int chun
   ab[c] = make_float2((float)a, (float)((double)beta[c] - mean * a));
 }
 
-template <bool RELU>
+template <int ACT>   // 0 none, 1 ReLU, 2 GELU (erf)
 __global__ void bn_apply_kernel(const __half* __restrict__ x, long long n_vec, int C, const float2* __restrict__ ab,
                                 __half* __restrict__ y) {
   griddep_launch_dependents();   // PDL: see ap_host.h::launch_pdl
@@ -100,9 +102,12 @@ __global__ void bn_apply_kernel(const __half* __restrict__ x, long long n_vec, i
       const float2 f = __half22float2(h2[j]);
       const float2 p0 = __ldg(ab + c0 + 2 * j), p1 = __ldg(ab + c0 + 2 * j + 1);
       float v0 = fmaf(f.x, p0.x, p0.y), v1 = fmaf(f.y, p1.x, p1.y);
-      if (RELU) {
+      if (ACT == 1) {
         v0 = fmaxf(v0, 0.f);
         v1 = fmaxf(v1, 0.f);
+      } else if (ACT == 2) {
+        v0 = gelu_erf(v0);
+        v1 = gelu_erf(v1);
       }
       o2[j] = __floats2half2_rn(v0, v1);
     }
@@ -203,10 +208,11 @@ static int launch_conv_direct(const void* x, const void* w, const float* bias, v
 using namespace ap;
 
 extern "C" int ap_batchnorm_train_nhwc_f16(const void* x, long long rows, int C, const float* gamma, const float* beta,
-                                           float eps, int relu, float* workspace, long long workspace_floats, void* out,
+                                           float eps, int act, float* workspace, long long workspace_floats, void* out,
                                            void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
   AP_REQUIRE(x && out && gamma && beta && workspace, "batchnorm: null pointer");
+  AP_REQUIRE(act >= AP_ACT_NONE && act <= AP_ACT_GELU, "batchnorm: activation %d is not one of AP_ACT_*", act);
   AP_REQUIRE(rows > 0 && C > 0 && C % 8 == 0 && C / 8 <= 256, "batchnorm: C=%d must be a multiple of 8, <= 2048", C);
   const int vecs = C / 8;
   int k = 256 / vecs;
@@ -230,8 +236,9 @@ extern "C" int ap_batchnorm_train_nhwc_f16(const void* x, long long rows, int C,
   const long long n_vec = rows * vecs;
   long long blocks = (n_vec + 255) / 256;
   if (blocks > num_sms() * 16LL) blocks = num_sms() * 16LL;
-  if (relu) AP_LAUNCH((bn_apply_kernel<true>), (unsigned)blocks, 256, 0, stream, (const __half*)x, n_vec, C, ab, (__half*)out);
-  else AP_LAUNCH((bn_apply_kernel<false>), (unsigned)blocks, 256, 0, stream, (const __half*)x, n_vec, C, ab, (__half*)out);
+  if (act == 1) AP_LAUNCH((bn_apply_kernel<1>), (unsigned)blocks, 256, 0, stream, (const __half*)x, n_vec, C, ab, (__half*)out);
+  else if (act == 2) AP_LAUNCH((bn_apply_kernel<2>), (unsigned)blocks, 256, 0, stream, (const __half*)x, n_vec, C, ab, (__half*)out);
+  else AP_LAUNCH((bn_apply_kernel<0>), (unsigned)blocks, 256, 0, stream, (const __half*)x, n_vec, C, ab, (__half*)out);
   AP_CHECK_CUDA(cudaGetLastError());
   return AP_OK;
 }

@@ -138,8 +138,9 @@ def _with_stats(out, rs, cs, row_stats, col_stats):
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, residual: torch.Tensor | None = None,
          a2: torch.Tensor | None = None, geglu: bool = False, out: torch.Tensor | None = None,
          bias_group_rows: int = 0, n_valid: int = 0, block_n: int = 0, out_f32: bool = False,
-         row_stats: bool = False, col_stats: bool = False, ln: LNFold | None = None):
+         row_stats: bool = False, col_stats: bool = False, ln: LNFold | None = None, gelu: bool = False):
     """out = [a | a2] @ w.T (+bias) (+residual); a:[M,K1] fp16 (row stride may exceed K1), w:[N,K1+K2] fp16.
+    gelu: out = gelu_erf(a @ w.T + bias) (AP_GEMM_GELU; not with a residual, GEGLU or `ln`).
     row_stats / col_stats: also return the epilogue's RowStats / ColStats of `out` (-> (out, RowStats?, ColStats?)).
     ln: fold a LayerNorm of `a` into this GEMM (see LNFold). bias may be a column slice of a wider fp32 table."""
     _ensure(a)
@@ -166,7 +167,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, res
         assert bias.is_contiguous() or bias.dim() == 2
     if residual is not None:
         assert residual.dtype == torch.float16 and residual.stride(1) == 1 and residual.shape[0] == M
-    flags = (1 if geglu else 0) | (2 if out_f32 else 0)
+    flags = (1 if geglu else 0) | (2 if out_f32 else 0) | (4 if gelu else 0)
     ext, rs, cs = _epilogue_ext(M, N, a.device, row_stats, col_stats, ln, bias, flags, K1 + K2, block_n)
     rc = lib().ap_gemm_f16(ptr(a), LL(a.stride(0)), I(K1), ptr(a2), LL(a2.stride(0) if a2 is not None else 0), I(K2),
                            ptr(w), LL(M), I(N), fptr(bias), LL(bias_group_rows), ptr(residual),
@@ -174,7 +175,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, res
                            I(nout), I(flags), I(block_n), stream_ptr(), _lib.ext_ptr(ext))
     check(rc, "ap_gemm_f16")
     if SHAPE_LOG is not None:
-        SHAPE_LOG.append(("gemm_geglu" if geglu else "gemm", M, N, K1 + K2, int(residual is not None)))
+        SHAPE_LOG.append(("gemm_geglu" if geglu else ("gemm_gelu" if gelu else "gemm"), M, N, K1 + K2,
+                          int(residual is not None)))
     _count()
     return _with_stats(out, rs, cs, row_stats, col_stats)
 
@@ -327,10 +329,18 @@ BN_MAX_BLOCKS = 2048  # AP_BN_MAX_BLOCKS in include/aniportrait_b200.h
 _bn_ws = {}
 
 
+ACTIVATIONS = {"none": 0, "relu": 1, "gelu": 2}   # AP_ACT_* in include/aniportrait_b200.h
+
+
 def batch_norm_train(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5, relu: bool = True,
-                     out: torch.Tensor | None = None) -> torch.Tensor:
-    """nn.BatchNorm2d in TRAIN mode (batch statistics over every row of the call, biased variance) + optional ReLU.
-    x: [..., C] fp16 channels-last, C % 8 == 0; gamma/beta fp32 [C]."""
+                     out: torch.Tensor | None = None, act: str | None = None) -> torch.Tensor:
+    """nn.BatchNorm2d in TRAIN mode (batch statistics over every row of the call, biased variance) + optional activation.
+    x: [..., C] fp16 channels-last, C % 8 == 0; gamma/beta fp32 [C]. act: "none", "relu" or "gelu" (erf); when not
+    given, `relu` chooses between ReLU and none."""
+    if act is None:
+        act = "relu" if relu else "none"
+    if act not in ACTIVATIONS:
+        raise ValueError(f"act {act!r} is not one of {list(ACTIVATIONS)}")
     _ensure(x)
     assert x.dtype == torch.float16 and x.is_contiguous()
     c = x.shape[-1]
@@ -344,7 +354,7 @@ def batch_norm_train(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, e
         ws = torch.empty(2 * 2048 * (BN_MAX_BLOCKS + 1), dtype=torch.float32, device=x.device)
         _bn_ws[key] = ws
     rc = lib().ap_batchnorm_train_nhwc_f16(ptr(x), LL(rows), I(c), fptr(gamma), fptr(beta), _lib.c_float(eps),
-                                           I(1 if relu else 0), fptr(ws), LL(ws.numel()), ptr(out), stream_ptr())
+                                           I(ACTIVATIONS[act]), fptr(ws), LL(ws.numel()), ptr(out), stream_ptr())
     check(rc, "ap_batchnorm_train_nhwc_f16")
     _count(3)
     return out
@@ -374,6 +384,79 @@ def conv2d_direct(x: torch.Tensor, w_packed: torch.Tensor, stride: int, pad: int
     rc = lib().ap_conv2d_direct_nhwc_f16(ptr(x), I(cin), I(nf), I(h), I(wd), ptr(w_packed), I(cout), I(k), I(stride),
                                          I(pad), fptr(bias), ptr(out), stream_ptr())
     check(rc, "ap_conv2d_direct_nhwc_f16")
+    _count()
+    return out
+
+
+# --------------------------------------------------------------------------------------------------------------
+# wav2vec2 audio encoder
+# --------------------------------------------------------------------------------------------------------------
+def conv1d_stem(wave: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
+    """Conv1d(1 -> Cout, kernel 10, stride 5, no bias) of an fp32 waveform [S] with fp32 weights [Cout, 10] (or the
+    module's [Cout, 1, 10]) -> fp16 [T0, Cout], T0 = (S - 10) // 5 + 1."""
+    _ensure(wave)
+    assert wave.dtype == torch.float32 and wave.is_contiguous() and wave.dim() == 1
+    w = w.reshape(w.shape[0], -1)
+    assert w.dtype == torch.float32 and w.is_contiguous() and w.shape[1] == 10
+    S, cout = wave.numel(), w.shape[0]
+    if S < 10:
+        raise ValueError(f"conv1d_stem: {S} samples give no output frame (need >= 10)")
+    out = torch.empty((S - 10) // 5 + 1, cout, dtype=torch.float16, device=wave.device)
+    check(lib().ap_conv1d_stem_f32(fptr(wave), LL(S), fptr(w), I(cout), ptr(out), stream_ptr()), "ap_conv1d_stem_f32")
+    _count()
+    return out
+
+
+def pack_conv1d_weight(w: torch.Tensor) -> torch.Tensor:
+    """Conv1d weight [Cout, Cin, k] -> [Cout, k*Cin] fp16, tap-major / channel-minor: a stride-2 conv over channels-last
+    frames x [T, Cin] is then a GEMM whose A row m is frames 2m .. 2m+k-1 (see conv1d_s2)."""
+    return w.permute(0, 2, 1).reshape(w.shape[0], -1).to(torch.float16).contiguous()
+
+
+def conv1d_s2(x: torch.Tensor, w_packed: torch.Tensor, k: int, gelu: bool = True) -> torch.Tensor:
+    """Conv1d(Cin -> Cout, kernel k in {2, 3}, stride 2, no padding) over x [T, Cin] fp16 (contiguous), as one GEMM
+    without an im2col buffer: A row m = frames (2m, 2m+1) read with row stride 2 Cin, plus for k = 3 the second source
+    frame 2m + 2 (a2 = x shifted by two frames, same row stride). Returns [(T - k) // 2 + 1, Cout] (GELU applied)."""
+    assert x.is_contiguous() and x.dim() == 2 and k in (2, 3)
+    T, c = x.shape
+    to = (T - k) // 2 + 1
+    if to < 1:
+        raise ValueError(f"conv1d_s2: {T} frames give no output for kernel {k}")
+    assert w_packed.shape[1] == k * c, (w_packed.shape, k, c)
+    pairs = x.as_strided((to, 2 * c), (2 * c, 1))
+    a2 = x[2:].as_strided((to, c), (2 * c, 1)) if k == 3 else None
+    return gemm(pairs, w_packed, a2=a2, gelu=gelu)
+
+
+def pack_pos_conv_weight(w: torch.Tensor) -> torch.Tensor:
+    """Grouped Conv1d weight [C, C / groups, K] (the weight norm already folded in) -> fp16 [C, K, C / groups]."""
+    return w.permute(0, 2, 1).to(torch.float16).contiguous()
+
+
+def pos_conv1d_gelu(x: torch.Tensor, w_packed: torch.Tensor, bias: torch.Tensor, groups: int) -> torch.Tensor:
+    """x + GELU(Conv1d(C, C, K, padding=K/2, groups)(x)[:-1] + bias) over x [T, C] fp16 (the positional convolution of
+    the wav2vec2 encoder with its SamePad trim and residual). w_packed from pack_pos_conv_weight; bias fp32 [C]."""
+    _ensure(x)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 2
+    T, c = x.shape
+    assert w_packed.dtype == torch.float16 and w_packed.is_contiguous() and w_packed.shape[0] == c
+    assert w_packed.shape[2] * groups == c and bias.dtype == torch.float32 and bias.numel() == c
+    out = torch.empty_like(x)
+    check(lib().ap_pos_conv1d_gelu_f16(ptr(x), LL(T), I(c), I(groups), I(w_packed.shape[1]), ptr(w_packed), fptr(bias),
+                                       ptr(out), stream_ptr()), "ap_pos_conv1d_gelu_f16")
+    _count()
+    return out
+
+
+def resample_rows_linear(x: torch.Tensor, t_out: int) -> torch.Tensor:
+    """F.interpolate(mode="linear", align_corners=True) along the rows of x [T_in, C] fp16 -> [t_out, C]."""
+    _ensure(x)
+    assert x.dtype == torch.float16 and x.is_contiguous() and x.dim() == 2
+    if t_out < 1:
+        raise ValueError(f"resample_rows_linear: t_out={t_out} must be >= 1")
+    out = torch.empty(t_out, x.shape[1], dtype=torch.float16, device=x.device)
+    check(lib().ap_resample_rows_linear_f16(ptr(x), LL(x.shape[0]), I(x.shape[1]), ptr(out), LL(t_out), stream_ptr()),
+          "ap_resample_rows_linear_f16")
     _count()
     return out
 

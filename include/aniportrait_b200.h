@@ -30,6 +30,7 @@ extern "C" {
 /* flags for ap_gemm_f16 */
 #define AP_GEMM_GEGLU 1 /* weight rows interleaved [16 value | 16 gate]; out = value * gelu_erf(gate), N/2 columns */
 #define AP_GEMM_OUT_F32 2 /* `out` is fp32 [M, ldo] (used for the small per-step bias tables) */
+#define AP_GEMM_GELU 4    /* out = gelu_erf(acc + bias) (wav2vec2 conv layers 1-6 and FFN up-projection); no residual */
 
 /*
  * Optional epilogue extensions of ap_gemm_f16 / ap_conv3x3_nhwc_f16 (pass NULL for none). They need the TMA epilogue
@@ -133,15 +134,20 @@ int ap_layernorm_f16(const void* x, long long rows, int C, float eps, const floa
                      const float* pe, int rows_per_pe, int pe_period, void* out, void* stream);
 
 /*
- * BatchNorm2d with BATCH statistics (train mode: biased variance over all `rows` = frames*H*W of the call) + optional ReLU,
- * channels-last. Replaces nn.BatchNorm2d + nn.ReLU of the PoseGuider, which the reference never switches to eval mode
- * (reference src/models/pose_guider.py:19-89; scripts/pose2vid.py:102-110). x/out: [rows, C] fp16, C % 8 == 0.
+ * BatchNorm2d with BATCH statistics (train mode: biased variance over all `rows` = frames*H*W of the call) + optional
+ * activation `act` (AP_ACT_*; 1 keeps the former `relu` flag's meaning), channels-last. Replaces nn.BatchNorm2d + nn.ReLU
+ * of the PoseGuider, which the reference never switches to eval mode (reference src/models/pose_guider.py:19-89;
+ * scripts/pose2vid.py:102-110), and, with AP_ACT_GELU, wav2vec2's GroupNorm(512, 512) + GELU after its first convolution
+ * (per-channel statistics over time for one clip). x/out: [rows, C] fp16, C % 8 == 0.
  * workspace: fp32, at least 2*C*(AP_BN_MAX_BLOCKS+1) floats (per-block partial sums, then the per-channel affine pair);
  * two-stage order-fixed reduction, double-precision finalize.
  */
 #define AP_BN_MAX_BLOCKS 2048
+#define AP_ACT_NONE 0
+#define AP_ACT_RELU 1
+#define AP_ACT_GELU 2
 int ap_batchnorm_train_nhwc_f16(const void* x, long long rows, int C, const float* gamma, const float* beta, float eps,
-                                int relu, float* workspace, long long workspace_floats, void* out, void* stream);
+                                int act, float* workspace, long long workspace_floats, void* out, void* stream);
 
 /*
  * Direct convolution for the PoseGuider stem's small channel counts (reference src/models/pose_guider.py:19-40):
@@ -151,6 +157,25 @@ int ap_batchnorm_train_nhwc_f16(const void* x, long long rows, int C, const floa
  */
 int ap_conv2d_direct_nhwc_f16(const void* x, int Cin, int Nf, int H, int W, const void* w, int Cout, int K, int stride,
                               int pad, const float* bias, void* out, void* stream);
+
+/*
+ * wav2vec2 audio encoder pieces that are not GEMM-shaped (transformers Wav2Vec2Model as the reference's
+ * src/audio_models/wav2vec2.py:30-64 runs it; the strided conv layers 1-6 are ap_gemm_f16 calls over frame pairs).
+ *
+ * ap_conv1d_stem_f32: feature-extractor layer 0, Conv1d(1 -> Cout, K = 10, stride 5, no bias) over an fp32 waveform
+ *   wave [samples]; w fp32 [Cout, 10]; out fp16 [T0, Cout], T0 = (samples - 10) / 5 + 1 >= 1, Cout % 64 == 0. fp32 math.
+ * ap_resample_rows_linear_f16: F.interpolate(mode="linear", align_corners=True) along the rows of x [T_in, C] ->
+ *   out [T_out, C] (C % 8 == 0); source row of output i = ((T_in - 1) / (T_out - 1)) * i in fp32, as torch computes it;
+ *   T_out = 1 reads row 0.
+ * ap_pos_conv1d_gelu_f16: the positional convolution of the encoder, out = x + GELU(conv(x) + bias) with
+ *   conv = Conv1d(C -> C, K, padding K/2, `groups` groups) over time, the last output dropped (SamePad, K even).
+ *   x/out [T, C] fp16 (out != x), C / groups == 48, K even and <= 256; w fp16 [C, K, C / groups] (tap-major, channel-minor:
+ *   the weight-normalised kernel folded once at load time); bias fp32 [C]. mma.sync, fixed summation order.
+ */
+int ap_conv1d_stem_f32(const float* wave, long long samples, const float* w, int Cout, void* out, void* stream);
+int ap_resample_rows_linear_f16(const void* x, long long T_in, int C, void* out, long long T_out, void* stream);
+int ap_pos_conv1d_gelu_f16(const void* x, long long T, int C, int groups, int K, const void* w, const float* bias,
+                           void* out, void* stream);
 
 /* Row softmax, fp16 in/out (may be in place), fp32 math: the VAE mid-block attention (single head, d = 512) is evaluated as
  * GEMM -> softmax -> GEMM (diffusers AutoencoderKL [dep], reference pipeline_pose2vid_long.py:118-121). */
