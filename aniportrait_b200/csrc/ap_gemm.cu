@@ -51,6 +51,7 @@ struct GemmParams {
   int n_valid;             // columns >= n_valid are not stored
   int out_f32;             // store fp32 instead of fp16 (small bias-table GEMMs)
   int gelu;                // AP_GEMM_GELU: out = gelu_erf(acc + bias) (never with a residual)
+  int quick_gelu;          // AP_GEMM_QUICK_GELU: out = quick_gelu(acc + bias) (same restrictions; never with gelu)
   // TMA epilogue (per-warp 32-row x 32-column boxes staged in 64B-swizzled shared memory)
   int tma_epi;             // 1: outputs leave through TMA stores, the residual arrives through TMA loads
   int sub_w, sub_h, sub_n; // conv modes: geometry of a warp's 32-row sub-box
@@ -363,6 +364,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CU
         if (p.gelu) {
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
+        } else if (p.quick_gelu) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = quick_gelu(v[j]);
         }
         if (has_res) {
           mbar_wait_quiet(rbar, rphase);
@@ -492,6 +496,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CU
       if (p.gelu) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
+      } else if (p.quick_gelu) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v[j] = quick_gelu(v[j]);
       }
       if (!row_ok) return;
       const bool vec_ok = (ncol + 32 <= p.n_valid) && ((p.ldo & 7) == 0);
@@ -722,6 +729,10 @@ extern "C" int ap_gemm_f16(const void* a, long long lda, int K1, const void* a2,
   p.gelu = (flags & AP_GEMM_GELU) ? 1 : 0;
   AP_REQUIRE(!p.gelu || (epi == EPI_LINEAR && residual == nullptr && !(ext && ext->ln_rstd)),
              "gemm: GELU epilogue is not available with GEGLU, a residual or LayerNorm folding");
+  p.quick_gelu = (flags & AP_GEMM_QUICK_GELU) ? 1 : 0;
+  AP_REQUIRE(!(p.gelu && p.quick_gelu), "gemm: AP_GEMM_GELU and AP_GEMM_QUICK_GELU are mutually exclusive");
+  AP_REQUIRE(!p.quick_gelu || (epi == EPI_LINEAR && residual == nullptr && !(ext && ext->ln_rstd)),
+             "gemm: quick-GELU epilogue is not available with GEGLU, a residual or LayerNorm folding");
 
   CUtensorMap tmA1, tmA2, tmB;
   {

@@ -138,9 +138,11 @@ def _with_stats(out, rs, cs, row_stats, col_stats):
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, residual: torch.Tensor | None = None,
          a2: torch.Tensor | None = None, geglu: bool = False, out: torch.Tensor | None = None,
          bias_group_rows: int = 0, n_valid: int = 0, block_n: int = 0, out_f32: bool = False,
-         row_stats: bool = False, col_stats: bool = False, ln: LNFold | None = None, gelu: bool = False):
+         row_stats: bool = False, col_stats: bool = False, ln: LNFold | None = None, gelu: bool = False,
+         quick_gelu: bool = False):
     """out = [a | a2] @ w.T (+bias) (+residual); a:[M,K1] fp16 (row stride may exceed K1), w:[N,K1+K2] fp16.
     gelu: out = gelu_erf(a @ w.T + bias) (AP_GEMM_GELU; not with a residual, GEGLU or `ln`).
+    quick_gelu: out = y * sigmoid(1.702 y), y = a @ w.T + bias (AP_GEMM_QUICK_GELU; same restrictions, not with gelu).
     row_stats / col_stats: also return the epilogue's RowStats / ColStats of `out` (-> (out, RowStats?, ColStats?)).
     ln: fold a LayerNorm of `a` into this GEMM (see LNFold). bias may be a column slice of a wider fp32 table."""
     _ensure(a)
@@ -167,7 +169,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, res
         assert bias.is_contiguous() or bias.dim() == 2
     if residual is not None:
         assert residual.dtype == torch.float16 and residual.stride(1) == 1 and residual.shape[0] == M
-    flags = (1 if geglu else 0) | (2 if out_f32 else 0) | (4 if gelu else 0)
+    flags = (1 if geglu else 0) | (2 if out_f32 else 0) | (4 if gelu else 0) | (8 if quick_gelu else 0)
     ext, rs, cs = _epilogue_ext(M, N, a.device, row_stats, col_stats, ln, bias, flags, K1 + K2, block_n)
     rc = lib().ap_gemm_f16(ptr(a), LL(a.stride(0)), I(K1), ptr(a2), LL(a2.stride(0) if a2 is not None else 0), I(K2),
                            ptr(w), LL(M), I(N), fptr(bias), LL(bias_group_rows), ptr(residual),
@@ -175,8 +177,8 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: torch.Tensor | None = None, res
                            I(nout), I(flags), I(block_n), stream_ptr(), _lib.ext_ptr(ext))
     check(rc, "ap_gemm_f16")
     if SHAPE_LOG is not None:
-        SHAPE_LOG.append(("gemm_geglu" if geglu else ("gemm_gelu" if gelu else "gemm"), M, N, K1 + K2,
-                          int(residual is not None)))
+        kind = "gemm_geglu" if geglu else ("gemm_gelu" if gelu else ("gemm_quick_gelu" if quick_gelu else "gemm"))
+        SHAPE_LOG.append((kind, M, N, K1 + K2, int(residual is not None)))
     _count()
     return _with_stats(out, rs, cs, row_stats, col_stats)
 
@@ -457,6 +459,29 @@ def resample_rows_linear(x: torch.Tensor, t_out: int) -> torch.Tensor:
     out = torch.empty(t_out, x.shape[1], dtype=torch.float16, device=x.device)
     check(lib().ap_resample_rows_linear_f16(ptr(x), LL(x.shape[0]), I(x.shape[1]), ptr(out), LL(t_out), stream_ptr()),
           "ap_resample_rows_linear_f16")
+    _count()
+    return out
+
+
+# --------------------------------------------------------------------------------------------------------------
+# CLIP vision encoder
+# --------------------------------------------------------------------------------------------------------------
+def patch_kpad(patch: int) -> int:
+    """Width of the patch-embedding GEMM operand: 3 P^2 pixel columns plus the CLS column, padded to a multiple of 64."""
+    return (3 * patch * patch + 1 + 63) // 64 * 64
+
+
+def patchify(pixels: torch.Tensor, patch: int) -> torch.Tensor:
+    """NCHW pixels [B, 3, H, W] (fp16 or fp32, contiguous) -> fp16 [B * (1 + Gh Gw), patch_kpad(patch)]: per image a CLS row
+    (1.0 in column 3 P^2) then the patches in flatten(2) order, columns (c, ky, kx), zero padded (ap_patchify_nchw_f16)."""
+    _ensure(pixels)
+    assert pixels.dim() == 4 and pixels.shape[1] == 3 and pixels.is_contiguous()
+    assert pixels.dtype in (torch.float16, torch.float32), pixels.dtype
+    B, _, H, W = pixels.shape
+    kpad = patch_kpad(patch)
+    out = torch.empty(B * (1 + (H // patch) * (W // patch)), kpad, dtype=torch.float16, device=pixels.device)
+    check(lib().ap_patchify_nchw_f16(ptr(pixels), I(1 if pixels.dtype == torch.float32 else 0), I(B), I(H), I(W),
+                                     I(patch), ptr(out), I(kpad), stream_ptr()), "ap_patchify_nchw_f16")
     _count()
     return out
 

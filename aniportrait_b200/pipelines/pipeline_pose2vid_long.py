@@ -25,6 +25,7 @@ import numpy as np
 import torch
 
 from .. import ops
+from ..models.clip_vision import kernels_enabled
 from ..models.mutual_self_attention import ReferenceAttentionControl
 from .sharding import plan_units, plan_windows, windows_of_rank
 from .image_processor import VaeImageProcessor
@@ -549,10 +550,12 @@ class Pose2VideoPipeline:
         static = bool(self.use_cuda_graph)
 
         if static:
+            # the last entry: clip_vision.enable_kernels rebinds the encoder's forward without touching its parameters, so
+            # the fingerprint does not see it; a session captured on the other CLIP path must not be replayed
             key = (L, h, w, dup, tuple(tuple(wd) for wd in my_windows), tuple(units), shard, rank, world,
                    self.group_units if shard else 0, clip_is_embed,
                    tuple(clip_in.shape), tuple(ref_image_tensor.shape), tuple(pose_cond.shape),
-                   self._weights_fingerprint())
+                   self._weights_fingerprint(), kernels_enabled(self.image_encoder))
             S = self._sessions.get(key)
             if S is None:
                 while len(self._sessions) >= self.max_sessions:     # each session pins ~10 GB of activations

@@ -31,6 +31,7 @@ extern "C" {
 #define AP_GEMM_GEGLU 1 /* weight rows interleaved [16 value | 16 gate]; out = value * gelu_erf(gate), N/2 columns */
 #define AP_GEMM_OUT_F32 2 /* `out` is fp32 [M, ldo] (used for the small per-step bias tables) */
 #define AP_GEMM_GELU 4    /* out = gelu_erf(acc + bias) (wav2vec2 conv layers 1-6 and FFN up-projection); no residual */
+#define AP_GEMM_QUICK_GELU 8 /* out = y * sigmoid(1.702 y), y = acc + bias (CLIP fc1); as AP_GEMM_GELU, never with it */
 
 /*
  * Optional epilogue extensions of ap_gemm_f16 / ap_conv3x3_nhwc_f16 (pass NULL for none). They need the TMA epilogue
@@ -176,6 +177,17 @@ int ap_conv1d_stem_f32(const float* wave, long long samples, const float* w, int
 int ap_resample_rows_linear_f16(const void* x, long long T_in, int C, void* out, long long T_out, void* stream);
 int ap_pos_conv1d_gelu_f16(const void* x, long long T, int C, int groups, int K, const void* w, const float* bias,
                            void* out, void* stream);
+
+/*
+ * CLIP vision patch embedding as a GEMM operand (transformers CLIPVisionEmbeddings: Conv2d(3, C, P, stride P, no bias),
+ * flatten(2), class token prepended). pixels: contiguous NCHW [B, 3, H, W], fp16 (in_f32 = 0) or fp32 (in_f32 = 1);
+ * H, W multiples of `patch`. out: fp16 [B * (1 + Gh * Gw), kpad], Gh = H / patch, Gw = W / patch. Row 0 of each image is
+ * the CLS row: zeros with a single 1.0 in column 3 * patch^2 (the packed weight holds class_embedding there); row 1 + i is
+ * patch i in row-major (flatten(2)) order, columns (c, ky, kx) as Conv2d.weight.reshape(C, -1), then zeros up to kpad.
+ * kpad % 64 == 0 and kpad > 3 * patch^2. Pure data movement: bit-exact.
+ */
+int ap_patchify_nchw_f16(const void* pixels, int in_f32, int B, int H, int W, int patch, void* out, int kpad,
+                         void* stream);
 
 /* Row softmax, fp16 in/out (may be in place), fp32 math: the VAE mid-block attention (single head, d = 512) is evaluated as
  * GEMM -> softmax -> GEMM (diffusers AutoencoderKL [dep], reference pipeline_pose2vid_long.py:118-121). */
