@@ -299,6 +299,8 @@ extern "C" int ap_attention_f16(const void* q, const void* k, const void* v, lon
   AP_REQUIRE(dpad == 64 || dpad == 128 || dpad == 192, "attention: dpad must be 64/128/192 (got %d)", dpad);
   AP_REQUIRE(head_dim % 8 == 0 && head_dim <= dpad, "attention: head_dim %d must be a multiple of 8 and <= dpad", head_dim);
   AP_REQUIRE(ld_qkv % 8 == 0 && ldo % 8 == 0, "attention: leading dims must be multiples of 8 elements");
+  // the epilogue stores __half2 pairs; q/k/v and the bank are checked by encode_tmap (16 B)
+  AP_REQUIRE((reinterpret_cast<uintptr_t>(out) & 3) == 0, "attention: out must be 4-byte aligned");
   AP_REQUIRE(n_frames > 0 && tokens > 0 && heads > 0, "attention: bad shape");
   const bool has_bank = bank_k != nullptr && bank_tokens > 0;
   AP_REQUIRE(!has_bank || (bank_v && frames_per_bank > 0 && first_bank_frame >= 0 && n_banks > 0),

@@ -588,6 +588,9 @@ extern "C" int ap_temporal_attention_f16(const void* qkv, long long ld, void* ou
   AP_REQUIRE(heads >= 1 && heads <= 8 && C % heads == 0, "temporal_attention: heads=%d unsupported", heads);
   const int d = C / heads;
   AP_REQUIRE(d % 8 == 0 && ld % 8 == 0 && ldo % 8 == 0, "temporal_attention: head_dim/ld must be multiples of 8");
+  // both kernels move q/k/v and out in 16-byte pieces (cp.async / uint4)
+  AP_REQUIRE((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
+             "temporal_attention: qkv and out must be 16-byte aligned");
   static const bool force_scalar = getenv("AP_TEMPORAL_SCALAR") != nullptr;   // A/B switch: the pre-MMA kernel
   if (!force_scalar && F <= 16 && C % TA_GC == 0 && heads * d == C && (d == 40 || d == 80 || d == 160)) {
     const unsigned grid = (unsigned)((long long)B * N * (C / TA_GC));

@@ -549,6 +549,8 @@ extern "C" int ap_layernorm_finalize_f16(const void* row_stat, int parts, long l
 
 extern "C" int ap_softmax_rows_f16(const void* x, void* out, long long rows, int cols, long long ld, void* stream) {
   AP_REQUIRE(x && out && cols % 2 == 0 && ld % 2 == 0, "softmax_rows: cols/ld must be even");
+  AP_REQUIRE((reinterpret_cast<uintptr_t>(x) & 3) == 0 && (reinterpret_cast<uintptr_t>(out) & 3) == 0,
+             "softmax_rows: x and out must be 4-byte aligned (__half2 accesses)");
   AP_LAUNCH((softmax_rows_kernel), (unsigned)rows, 256, 0, (cudaStream_t)stream, (const __half*)x, (__half*)out, cols, ld);
   AP_CHECK_CUDA(cudaGetLastError());
   return AP_OK;

@@ -190,7 +190,8 @@ int ap_patchify_nchw_f16(const void* pixels, int in_f32, int B, int H, int W, in
                          void* stream);
 
 /* Row softmax, fp16 in/out (may be in place), fp32 math: the VAE mid-block attention (single head, d = 512) is evaluated as
- * GEMM -> softmax -> GEMM (diffusers AutoencoderKL [dep], reference pipeline_pose2vid_long.py:118-121). */
+ * GEMM -> softmax -> GEMM (diffusers AutoencoderKL [dep], reference pipeline_pose2vid_long.py:118-121).
+ * x/out: rows of ld elements, only the first cols are read and written; cols and ld even, x and out 4-byte aligned. */
 int ap_softmax_rows_f16(const void* x, void* out, long long rows, int cols, long long ld, void* stream);
 
 /*
@@ -198,6 +199,7 @@ int ap_softmax_rows_f16(const void* x, void* out, long long rows, int cols, long
  * at columns [h*dpad, h*dpad + head_dim) (zero padded to dpad in {64,128,192}); frames >= first_bank_frame also attend
  * to bank (frame - first_bank_frame) / frames_per_bank of bank_k/bank_v: [n_banks*bank_tokens, ld_bank] (NULL = none).
  * out: [n_frames*tokens, ldo], head h at columns [h*head_dim, (h+1)*head_dim).
+ * head_dim % 8 == 0, ld_qkv and ldo multiples of 8; q/k/v/bank 16-byte aligned, out 4-byte aligned.
  * Replaces F.scaled_dot_product_attention under ReferenceAttentionControl's read-mode forward, including the CFG
  * redo for the unconditional half (reference src/models/mutual_self_attention.py:147-186; src/models/attention.py:323-330).
  */
@@ -209,6 +211,7 @@ int ap_attention_f16(const void* q, const void* k, const void* v, long long ld_q
 /*
  * Temporal attention core of the motion module: softmax over the F frames of each (batch, position, head).
  * qkv: [B*F*N, ld] = [q | k | v] (C columns each, token row (b*F+f)*N+p); out: [B*F*N, ldo].
+ * 1 <= F <= 32, heads <= 8, C / heads % 8 == 0, ld and ldo multiples of 8; qkv and out 16-byte aligned.
  * Replaces VersatileAttention's rearrange + SDPA + rearrange (reference src/models/motion_module.py:351-388).
  */
 int ap_temporal_attention_f16(const void* qkv, long long ld, void* out, long long ldo, int B, int F, int N, int C,
