@@ -82,6 +82,16 @@ class EpilogueExt(ctypes.Structure):
                 ("col_stat_ld", c_longlong), ("ln_rstd", c_void_p), ("bias_ld", c_longlong)]
 
 
+class PoseDecoderParams(ctypes.Structure):
+    """ap_pose_decoder_params of include/aniportrait_b200.h."""
+    _fields_ = [("layers", c_int), ("out_dim", c_int), ("embed_dim", c_int), ("heads", c_int), ("ffn_dim", c_int),
+                ("mask_len", c_int), ("pe_len", c_int), ("eps", c_float),
+                ("w_qkv", c_void_p), ("w_out", c_void_p), ("w_ff1", c_void_p), ("w_ff2", c_void_p), ("vec", c_void_p),
+                ("pose_map_w", c_void_p), ("pose_map_b", c_void_p), ("pose_map_r_w", c_void_p),
+                ("pose_map_r_b", c_void_p), ("pe", c_void_p), ("id_row", c_void_p), ("mask", c_void_p),
+                ("cross", c_void_p)]
+
+
 def ext_ptr(ext):
     """NULL or a pointer to an EpilogueExt (the struct is copied by the callee before it returns)."""
     if ext is None:

@@ -217,10 +217,13 @@ def mesh_infer(model, enc_cache: PackedCache, head_cache: PackedCache, input_val
 
 
 def enable_kernels(model):
-    """Run `model.audio_encoder` (and, for an Audio2MeshModel, its in_fn / out_fn head) on the library's kernels.
+    """Run `model.audio_encoder` and `model.infer` on the library's kernels.
 
-    model: an instance of the reference's Audio2MeshModel (has in_fn / out_fn, no decoder) or Audio2PoseModel (has
-    transformer_decoder; composes with enable_kv_cache in either order). Only bound methods on the instances change."""
+    model: an instance of the reference's Audio2MeshModel (has in_fn / out_fn, no decoder: `infer` runs the in_fn / out_fn
+    head as two GEMMs) or Audio2PoseModel (has transformer_decoder: `infer` runs the encoder, the folded cross-attention
+    GEMM and the one-launch decoder of pose_decoder.py). Only bound methods on the instances change. For an
+    Audio2PoseModel, `enable_kv_cache` also rebinds `infer`: whichever of the two was applied last decides which `infer`
+    runs (the encoder stays on the kernels either way)."""
     enc = getattr(model, "audio_encoder", None)
     if enc is None or not hasattr(enc, "config"):
         raise TypeError(f"enable_kernels: {type(model).__name__} has no wav2vec2 audio_encoder")
@@ -241,5 +244,11 @@ def enable_kernels(model):
 
         def infer(self, input_value, seq_len):
             return mesh_infer(self, enc_cache, head_cache, input_value, seq_len)
-        model.infer = types.MethodType(infer, model)
+    else:
+        from .pose_decoder import PoseDecoder
+        decoder = PoseDecoder(model)
+
+        def infer(self, input_value, seq_len, id_seed=None):
+            return decoder.infer(enc_cache, input_value, seq_len, id_seed)
+    model.infer = types.MethodType(infer, model)
     return model

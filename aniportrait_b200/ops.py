@@ -697,3 +697,54 @@ def pack_frames_u8(video: torch.Tensor, rescale: bool = False) -> torch.Tensor:
                                   stream_ptr()), "ap_pack_frames_u8")
     _count()
     return out
+
+
+# --------------------------------------------------------------------------------------------------------------
+# Audio2Pose head-pose decoder
+# --------------------------------------------------------------------------------------------------------------
+POSE_VEC = 6656          # AP_POSE_VEC: per-layer fp32 vector (biases, then the three LayerNorms' weight and bias)
+POSE_E, POSE_HEADS, POSE_FFN = 512, 8, 1024
+
+
+def pose_decoder(layers: dict, pose_map_w: torch.Tensor, pose_map_b: torch.Tensor, pose_map_r_w: torch.Tensor,
+                 pose_map_r_b: torch.Tensor, pe: torch.Tensor, mask: torch.Tensor, id_row: torch.Tensor,
+                 cross: torch.Tensor, T: int, eps: float) -> torch.Tensor:
+    """All T steps of the autoregressive pose decoder in one launch (ap_pose_decoder_f16) -> fp32 [T, out_dim].
+    layers: w_qkv / w_out / w_ff1 / w_ff2 fp16 [L, 1536 | 512 | 1024 | 512, 512 | 512 | 512 | 1024], vec fp32 [L, POSE_VEC];
+    pose_map_w fp32 [512, out_dim], pose_map_r_w [out_dim, 512]; pe fp32 [pe_len, 512]; mask fp32 [8, n, n];
+    id_row fp32 [512]; cross fp32 [T, L * 512]."""
+    _ensure(cross)
+    w_qkv, w_out, w_ff1, w_ff2, vec = (layers[k] for k in ("w_qkv", "w_out", "w_ff1", "w_ff2", "vec"))
+    L = w_qkv.shape[0]
+    for t, shape in ((w_qkv, (L, 3 * POSE_E, POSE_E)), (w_out, (L, POSE_E, POSE_E)), (w_ff1, (L, POSE_FFN, POSE_E)),
+                     (w_ff2, (L, POSE_E, POSE_FFN))):
+        assert t.dtype == torch.float16 and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape, shape)
+    od = pose_map_r_w.shape[0]
+    f32s = ((vec, (L, POSE_VEC)), (pose_map_w, (POSE_E, od)), (pose_map_b, (POSE_E,)), (pose_map_r_w, (od, POSE_E)),
+            (pose_map_r_b, (od,)), (id_row, (POSE_E,)), (cross, (T, L * POSE_E)))
+    for t, shape in f32s:
+        assert t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape, shape)
+    assert pe.dtype == torch.float32 and pe.is_contiguous() and pe.dim() == 2 and pe.shape[1] == POSE_E
+    assert mask.dtype == torch.float32 and mask.is_contiguous() and mask.dim() == 3 and mask.shape[1] == mask.shape[2]
+    prm = _lib.PoseDecoderParams(layers=L, out_dim=od, embed_dim=POSE_E, heads=mask.shape[0], ffn_dim=POSE_FFN,
+                                 mask_len=mask.shape[1], pe_len=pe.shape[0], eps=eps,
+                                 w_qkv=w_qkv.data_ptr(), w_out=w_out.data_ptr(), w_ff1=w_ff1.data_ptr(),
+                                 w_ff2=w_ff2.data_ptr(), vec=vec.data_ptr(), pose_map_w=pose_map_w.data_ptr(),
+                                 pose_map_b=pose_map_b.data_ptr(), pose_map_r_w=pose_map_r_w.data_ptr(),
+                                 pose_map_r_b=pose_map_r_b.data_ptr(), pe=pe.data_ptr(), id_row=id_row.data_ptr(),
+                                 mask=mask.data_ptr(), cross=cross.data_ptr())
+    kv = torch.empty(L, 2, POSE_HEADS, T, POSE_E // POSE_HEADS, dtype=torch.float16, device=cross.device)
+    out = torch.empty(T, od, dtype=torch.float32, device=cross.device)
+    check(lib().ap_pose_decoder_f16(_lib.ctypes.byref(prm), I(T), ptr(kv), fptr(out), stream_ptr()),
+          "ap_pose_decoder_f16")
+    _count()
+    return out
+
+
+def pose_decoder_ctas(device: int = 0) -> int:
+    """CTAs of the pose decoder's cluster on `device` (16, or 8 where 16 cannot be co-scheduled), chosen once."""
+    _lib.init(device)
+    n = _lib.c_int(0)
+    with torch.cuda.device(device):
+        check(lib().ap_pose_decoder_ctas(_lib.ctypes.byref(n)), "ap_pose_decoder_ctas")
+    return n.value

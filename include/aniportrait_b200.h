@@ -189,6 +189,70 @@ int ap_pos_conv1d_gelu_f16(const void* x, long long T, int C, int groups, int K,
 int ap_patchify_nchw_f16(const void* pixels, int in_f32, int B, int H, int W, int patch, void* out, int kpad,
                          void* stream);
 
+/*
+ * The autoregressive head-pose decoder of Audio2PoseModel.infer (reference src/audio_models/pose_model.py:97-124: an
+ * nn.TransformerDecoder of post-norm layers re-run over all pose tokens once per frame), in its incremental form: all T
+ * steps of one chunk in ONE launch, writing the fp32 poses out[T, out_dim]. For position i = 0 .. T-1:
+ *   x = token + (pe[i] + id_row), token = pose_map_b at i = 0, else pose_map(pose[i-1]);
+ *   per layer l: q, k, v = in_proj(x); k, v -> kv_cache row i; a = softmax(q.K^T / 8 + mask[h, i, 0..i]) . V per head;
+ *                x = LN1(x + out_proj(a)); x = LN2(x + cross[i, l]); x = LN3(x + linear2(relu(linear1(x))));
+ *   pose[i] = pose_map_r(x).
+ * cross is the one-key cross-attention out_proj(v_proj(memory_i)), computed for every frame before the call.
+ * Geometry: embed_dim 512, 8 heads of 64, ffn_dim 1024, ReLU, any layers >= 1, 1 <= out_dim <= 8,
+ *   1 <= T <= min(mask_len, pe_len, 1024); anything else returns AP_ERR_INVALID.
+ * Operands (all device pointers, row-major, contiguous):
+ *   w_qkv fp16 [layers, 1536, 512] (in_proj_weight), w_out fp16 [layers, 512, 512], w_ff1 fp16 [layers, 1024, 512],
+ *   w_ff2 fp16 [layers, 512, 1024].
+ *   vec fp32 [layers, AP_POSE_VEC]: per layer in_proj bias | out_proj bias | linear1 bias | linear2 bias | norm1 weight,
+ *   bias | norm2 weight, bias | norm3 weight, bias at the AP_POSE_* offsets; eps: the LayerNorms' epsilon (all equal).
+ *   pose_map_w fp32 [512, out_dim], pose_map_b [512], pose_map_r_w [out_dim, 512], pose_map_r_b [out_dim];
+ *   pe fp32 [pe_len, 512]; id_row fp32 [512] (the identity embedding's row); mask fp32 [8, mask_len, mask_len] (only
+ *   entries j <= i of row i are read); cross fp32 [T, layers * 512] (layer l at columns l * 512).
+ *   kv_cache: caller-owned fp16 [layers, 2, 8, T, 64] (k then v), overwritten; out fp32 [T, out_dim].
+ *   The four weights, vec, cross and kv_cache 16-byte aligned (they are read by bulk copies / 16-byte loads); the other
+ *   operands 4-byte aligned.
+ * Numerics: fp16 weights and KV cache, fp32 everything else; fixed reduction order, no atomics (bit-reproducible).
+ * The grid is one thread-block cluster of 16 CTAs (8 where the device cannot co-schedule 16), one SM each (about 222 KB of
+ * shared memory per CTA), chosen once per device at the first call; ap_pose_decoder_ctas reports the choice (and makes it
+ * if not made yet).
+ */
+#define AP_POSE_VEC 6656
+#define AP_POSE_B_QKV 0
+#define AP_POSE_B_OUT 1536
+#define AP_POSE_B_FF1 2048
+#define AP_POSE_B_FF2 3072
+#define AP_POSE_LN1_G 3584
+#define AP_POSE_LN1_B 4096
+#define AP_POSE_LN2_G 4608
+#define AP_POSE_LN2_B 5120
+#define AP_POSE_LN3_G 5632
+#define AP_POSE_LN3_B 6144
+typedef struct ap_pose_decoder_params {
+  int layers;
+  int out_dim;
+  int embed_dim;
+  int heads;
+  int ffn_dim;
+  int mask_len;
+  int pe_len;
+  float eps;
+  const void* w_qkv;
+  const void* w_out;
+  const void* w_ff1;
+  const void* w_ff2;
+  const float* vec;
+  const float* pose_map_w;
+  const float* pose_map_b;
+  const float* pose_map_r_w;
+  const float* pose_map_r_b;
+  const float* pe;
+  const float* id_row;
+  const float* mask;
+  const float* cross;
+} ap_pose_decoder_params;
+int ap_pose_decoder_f16(const ap_pose_decoder_params* params, int T, void* kv_cache, float* out, void* stream);
+int ap_pose_decoder_ctas(int* ctas);
+
 /* Row softmax, fp16 in/out (may be in place), fp32 math: the VAE mid-block attention (single head, d = 512) is evaluated as
  * GEMM -> softmax -> GEMM (diffusers AutoencoderKL [dep], reference pipeline_pose2vid_long.py:118-121).
  * x/out: rows of ld elements, only the first cols are read and written; cols and ld even, x and out 4-byte aligned. */
