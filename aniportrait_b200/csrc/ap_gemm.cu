@@ -39,7 +39,7 @@ struct GemmParams {
   int Nf, Ho, Wo;
   int bw, bh, bn;
   int tiles_x, tiles_y;
-  int C1;                  // channels of source 1 (A_CONV_S2 merged (phase, channel) coordinate)
+  int C1, C2;              // channels of source 1 / 2 (A_CONV_S2: each source's merged (phase, channel) coordinate)
   // epilogue
   const float* bias;       // [groups, Nout] fp32 or null
   int bias_group_rows;     // rows sharing one bias row (>= M -> single row)
@@ -48,6 +48,7 @@ struct GemmParams {
   int ldr;
   __half* out;             // [M, ldo]
   int ldo;
+  int out_al16, res_al16;  // out / residual base 16-byte aligned: the direct epilogue may use 16-byte vector accesses
   int n_valid;             // columns >= n_valid are not stored
   int out_f32;             // store fp32 instead of fp16 (small bias-table GEMMs)
   int gelu;                // AP_GEMM_GELU: out = gelu_erf(acc + bias) (never with a residual)
@@ -186,7 +187,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CU
               // input pixel = 2*o + k - 1  ->  k=0: (o-1, phase 1), k=1: (o, phase 0), k=2: (o, phase 1)
               const int px = (kx == 1) ? 0 : 1, dx = (kx == 0) ? -1 : 0;
               const int py = (ky == 1) ? 0 : 1, dy = (ky == 0) ? -1 : 0;
-              tma_load_5d(am, &full_bar[stage], a_dst, px * p.C1 + c0, x0 + dx, py, y0 + dy, n0);
+              tma_load_5d(am, &full_bar[stage], a_dst, px * (second ? p.C2 : p.C1) + c0, x0 + dx, py, y0 + dy, n0);
             }
             if (load_b) tma_load_2d(&tmB, &full_bar[stage], b_dst, kb * Cfg::BK, n_tile * BN);
           }
@@ -468,7 +469,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CU
               o[j] = __floats2half2_rn(a0, a1);
             }
             __half* dst = p.out + m * p.ldo + ocol;
-            if (ocol + 16 <= p.n_valid && (p.ldo & 7) == 0) {
+            if (ocol + 16 <= p.n_valid && (p.ldo & 7) == 0 && p.out_al16) {
               uint4* d4 = reinterpret_cast<uint4*>(dst);
               d4[0] = *reinterpret_cast<uint4*>(&o[0]);
               d4[1] = *reinterpret_cast<uint4*>(&o[4]);
@@ -501,9 +502,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CU
         for (int j = 0; j < 32; ++j) v[j] = quick_gelu(v[j]);
       }
       if (!row_ok) return;
-      const bool vec_ok = (ncol + 32 <= p.n_valid) && ((p.ldo & 7) == 0);
+      const bool vec_ok = (ncol + 32 <= p.n_valid) && ((p.ldo & 7) == 0) && p.out_al16;
       if (p.residual != nullptr) {
-        if (vec_ok && (p.ldr & 7) == 0) {
+        if (ncol + 32 <= p.n_valid && (p.ldr & 7) == 0 && p.res_al16) {
           const uint4* r4 = reinterpret_cast<const uint4*>(p.residual + m * p.ldr + ncol);
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
@@ -646,11 +647,17 @@ static int apply_ext(GemmParams& p, const ap_epilogue_ext* ext, int epi, long lo
   p.bias_ld = p.N;
   static const int epi_double = getenv("AP_GEMM_EPI_DOUBLE") ? atoi(getenv("AP_GEMM_EPI_DOUBLE")) : 1;
   p.epi_double = epi_double;
+  if (ext != nullptr && ext->bias_ld > 0) p.bias_ld = ext->bias_ld;
+  // both epilogues read the bias as float4: every bias row must start on a 16-byte boundary
+  if (p.bias != nullptr && ((reinterpret_cast<uintptr_t>(p.bias) & 15) != 0 || (p.bias_ld & 3) != 0))
+    return fail(AP_ERR_INVALID, "gemm: bias must be 16-byte aligned with bias_ld %% 4 == 0 (bias_ld %lld)", p.bias_ld);
   if (ext == nullptr) return AP_OK;
-  if (ext->bias_ld > 0) p.bias_ld = ext->bias_ld;
   const bool any = ext->row_stat_out || ext->col_stat_out || ext->ln_rstd;
   if (!any) return AP_OK;
   if (!p.tma_epi) return fail(AP_ERR_INVALID, "gemm: epilogue statistics / LayerNorm folding need the TMA epilogue (aligned fp16 out)");
+  // the partials sum what the epilogue computed, not what the clipped TMA store kept: only whole-width outputs
+  if ((ext->row_stat_out || ext->col_stat_out) && p.n_valid < (epi == EPI_GEGLU ? p.N / 2 : p.N))
+    return fail(AP_ERR_INVALID, "gemm: row / column statistics need n_valid (%d) == the output width", p.n_valid);
   if (ext->row_stat_out) {
     if (epi != EPI_LINEAR) return fail(AP_ERR_INVALID, "gemm: row statistics are not available with GEGLU");
     if (ext->row_stat_ld < m_pad) return fail(AP_ERR_INVALID, "gemm: row_stat_ld %lld < padded M %lld", ext->row_stat_ld, m_pad);
@@ -755,8 +762,10 @@ extern "C" int ap_gemm_f16(const void* a, long long lda, int K1, const void* a2,
   if (rc) return rc;
   // TMA epilogue whenever the output (and residual) satisfy TMA's 16-byte rules
   CUtensorMap tmOut = tmB, tmRes = tmB;
-  const bool aligned_out = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (ldo % 8) == 0 && (p.n_valid % 8) == 0;
-  const bool aligned_res = residual == nullptr || ((reinterpret_cast<uintptr_t>(residual) & 15) == 0 && (ldr % 8) == 0);
+  p.out_al16 = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+  p.res_al16 = (reinterpret_cast<uintptr_t>(residual) & 15) == 0;
+  const bool aligned_out = p.out_al16 && (ldo % 8) == 0 && (p.n_valid % 8) == 0;
+  const bool aligned_res = residual == nullptr || (p.res_al16 && (ldr % 8) == 0);
   static const bool no_tma_epi = getenv("AP_GEMM_NO_TMA_EPI") != nullptr;
   if (!p.out_f32 && aligned_out && aligned_res && !no_tma_epi) {
     const uint64_t dims[2] = {(uint64_t)p.n_valid, (uint64_t)M};
@@ -806,6 +815,7 @@ extern "C" int ap_conv3x3_nhwc_f16(const void* x, int C1, const void* x2, int C2
   p.kb_src2 = x2 ? C2 / 64 : 0;
   p.num_kb = 9 * (p.kb_src1 + p.kb_src2);
   p.C1 = C1;
+  p.C2 = x2 ? C2 : 0;
   p.bias = bias;
   p.bias_group_rows = (int)(bias_group_rows > 0 ? (bias_group_rows > 0x7fffffff ? 0x7fffffff : bias_group_rows)
                                                 : 0x7fffffff);
@@ -842,8 +852,10 @@ extern "C" int ap_conv3x3_nhwc_f16(const void* x, int C1, const void* x2, int C2
   rc = make_weight_map(&tmB, w, Cout, 9ll * (C1 + (x2 ? C2 : 0)), bn_);
   if (rc) return rc;
   CUtensorMap tmOut = tmB, tmRes = tmB;
-  const bool aligned_out = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (ldo % 8) == 0 && (p.n_valid % 8) == 0;
-  const bool aligned_res = residual == nullptr || (reinterpret_cast<uintptr_t>(residual) & 15) == 0;
+  p.out_al16 = (reinterpret_cast<uintptr_t>(out) & 15) == 0;
+  p.res_al16 = (reinterpret_cast<uintptr_t>(residual) & 15) == 0;
+  const bool aligned_out = p.out_al16 && (ldo % 8) == 0 && (p.n_valid % 8) == 0;
+  const bool aligned_res = residual == nullptr || p.res_al16;
   static const bool no_tma_epi = getenv("AP_GEMM_NO_TMA_EPI") != nullptr;
   if (aligned_out && aligned_res && !no_tma_epi) {
     p.sub_w = bw < 32 ? bw : 32;

@@ -44,6 +44,8 @@ extern "C" {
  *                 parts = 2 * ap_gemm_row_stat_parts(...) ; row_stat_ld >= M rounded up to 128
  *   col_stat_out  fp32 pairs per output column over 32 consecutive rows: [ceil(M / 128) * 4][col_stat_ld]
  *                 (conv: 32-row sub-boxes of the output tile; needs Ho * Wo % 32 == 0 so that no sub-box spans two frames)
+ *   Both need n_valid equal to the output width (N, N / 2 with GEGLU): the partials would otherwise include columns the
+ *   store clips. Refused (AP_ERR_INVALID) otherwise.
  * LayerNorm folded into this GEMM: A = [x | a2] with a2 = the [M, 8] fp16 matrix written by ap_layernorm_finalize_f16
  * (columns -mean_hi, -mean_lo, -mean_hi, 0...), weights [W diag(gamma) | colsum_hi, colsum_hi, colsum_lo, 0...] (K1 + 8
  * columns), `bias` = beta.W^T + b; the accumulator then holds x.W'^T - mean colsum(W') and the epilogue applies
@@ -71,8 +73,10 @@ int ap_init(int device);
  *   src/models/motion_module.py:122,144,163-170,233; src/models/resnet.py:207-209 (1x1 conv_shortcut, two-source
  *   K = torch.cat([hidden, skip]) of src/models/unet_3d_blocks.py:697,826 without materialising the concat).
  * a/a2: row-major fp16, leading dims lda/lda2 (elements); a2 may be NULL. w: [N, K1+K2] row-major contiguous.
- * bias: fp32 [groups, N] or NULL; output row m uses bias row m / bias_group_rows (<=0: one shared row).
+ * bias: fp32 [groups, N] or NULL; output row m uses bias row m / bias_group_rows (<=0: one shared row). The bias is read
+ *   as float4: its base must be 16-byte aligned and its row stride (ext->bias_ld, default N) a multiple of 4 floats.
  * residual: fp16 [M, ldr] or NULL. n_valid: columns >= n_valid are not written (<=0: all).
+ * out / residual of any 2-byte alignment are accepted; bases that are not 16-byte aligned take the direct-store epilogue.
  * block_n: 0 = auto (N must be a multiple of 32).
  */
 int ap_gemm_f16(const void* a, long long lda, int K1, const void* a2, long long lda2, int K2, const void* w,
@@ -86,7 +90,8 @@ int ap_gemm_row_stat_parts(long long M, int N, int K, int flags, int block_n);
  * 3x3 convolution, zero padding 1, stride 1|2, channels-last fp16, as an implicit GEMM (no im2col buffer).
  * Replaces InflatedConv3d / Downsample3D / Upsample3D.conv (reference src/models/resnet.py:10-18,52,107,166,195)
  * and conv_in/conv_out (src/models/unet_3d.py:90,250).
- * x: [Nf, H, W, C1]; x2: optional [Nf, H, W, C2] concatenated after x along channels; C1, C2 multiples of 64.
+ * x: [Nf, H, W, C1]; x2: optional [Nf, H, W, C2] concatenated after x along channels; C1, C2 multiples of 64, C1 != C2
+ * allowed, at stride 1 and 2. bias: as for ap_gemm_f16 (16-byte aligned, bias_ld % 4 == 0).
  * w: [Cout, 3, 3, C1+C2] (tap-major, channel-minor) fp16. out/residual: [Nf, H/stride, W/stride, ldo].
  */
 int ap_conv3x3_nhwc_f16(const void* x, int C1, const void* x2, int C2, int Nf, int H, int W, int stride,
