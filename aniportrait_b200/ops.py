@@ -700,6 +700,59 @@ def pack_frames_u8(video: torch.Tensor, rescale: bool = False) -> torch.Tensor:
 
 
 # --------------------------------------------------------------------------------------------------------------
+# Face-mesh projection and landmark pose frames
+# --------------------------------------------------------------------------------------------------------------
+LMK_CANVAS = 512       # AP_LMK_CANVAS
+LMK_MAX_EDGES = 255    # AP_LMK_MAX_EDGES
+
+
+def project_points(base: torch.Tensor, matrices: torch.Tensor, proj, width: float, height: float,
+                   offsets: torch.Tensor | None = None) -> torch.Tensor:
+    """fp64 pixel coordinates [L, N, 2] of base fp64 [N, 3] or [L, N, 3] (+ offsets fp32 [L, N, 3], added in fp64) under
+    the per-frame fp64 matrices [L, 4, 4] and the projection `proj` (16 host floats, row-major P): ap_project_points_f64."""
+    _ensure(matrices)
+    L = matrices.shape[0]
+    N = base.shape[-2]
+    assert matrices.dtype == torch.float64 and matrices.is_contiguous() and tuple(matrices.shape) == (L, 4, 4)
+    assert base.dtype == torch.float64 and base.is_contiguous() and base.device == matrices.device
+    assert tuple(base.shape) in ((N, 3), (L, N, 3)), base.shape
+    if offsets is not None:
+        assert offsets.dtype == torch.float32 and offsets.is_contiguous() and tuple(offsets.shape) == (L, N, 3)
+        assert offsets.device == matrices.device
+    p = (_lib.ctypes.c_double * 16)(*[float(v) for v in proj])
+    out = torch.empty(L, N, 2, dtype=torch.float64, device=matrices.device)
+    dp = _lib.ctypes.POINTER(_lib.ctypes.c_double)
+    check(lib().ap_project_points_f64(fptr(offsets), _lib.ctypes.cast(ptr(base), dp), I(1 if base.dim() == 3 else 0),
+                                      _lib.ctypes.cast(ptr(matrices), dp), p, I(L), I(N),
+                                      _lib.ctypes.c_double(width), _lib.ctypes.c_double(height),
+                                      _lib.ctypes.cast(ptr(out), dp), stream_ptr()), "ap_project_points_f64")
+    _count()
+    return out
+
+
+def draw_landmarks(keypoints: torch.Tensor, size_x: float, size_y: float, normed: bool, edges, colors,
+                   thickness: int = 2) -> torch.Tensor:
+    """Landmark pose frames uint8 [L, 512, 512, 3] of fp64 keypoints [L, N, 2] in one launch (ap_draw_landmarks_u8).
+    edges: int32 [E, 2] and colors: uint8 [E, 3] host arrays in draw order (numpy or CPU tensors)."""
+    import numpy as np
+    _ensure(keypoints)
+    assert keypoints.dtype == torch.float64 and keypoints.is_contiguous() and keypoints.dim() == 3
+    assert keypoints.shape[2] == 2
+    L, N, _ = keypoints.shape
+    e = np.ascontiguousarray(edges, dtype=np.int32).reshape(-1, 2)
+    c = np.ascontiguousarray(colors, dtype=np.uint8).reshape(-1, 3)
+    assert len(e) == len(c)
+    out = torch.empty(L, LMK_CANVAS, LMK_CANVAS, 3, dtype=torch.uint8, device=keypoints.device)
+    check(lib().ap_draw_landmarks_u8(_lib.ctypes.cast(ptr(keypoints), _lib.ctypes.POINTER(_lib.ctypes.c_double)), I(L),
+                                     I(N), _lib.ctypes.c_double(size_x), _lib.ctypes.c_double(size_y),
+                                     I(1 if normed else 0), e.ctypes.data_as(_lib.ctypes.POINTER(_lib.ctypes.c_int)),
+                                     c.ctypes.data_as(_lib.ctypes.POINTER(_lib.ctypes.c_ubyte)), I(len(e)),
+                                     I(thickness), ptr(out), stream_ptr()), "ap_draw_landmarks_u8")
+    _count()
+    return out
+
+
+# --------------------------------------------------------------------------------------------------------------
 # Audio2Pose head-pose decoder
 # --------------------------------------------------------------------------------------------------------------
 POSE_VEC = 6656          # AP_POSE_VEC: per-layer fp32 vector (biases, then the three LayerNorms' weight and bias)

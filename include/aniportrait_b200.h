@@ -324,6 +324,35 @@ int ap_cfg_ddim_step_f16(float* acc, const float* inv_count, int cfg, float guid
 int ap_pack_frames_u8(const void* video, const long long* strides, int B, int F, int H, int W, int rescale, void* out,
                       void* stream);
 
+/*
+ * Face-mesh projection to pixels, the per-point part of pose_util.project_points / project_points_with_trans (reference
+ * src/utils/pose_util.py:30-59). For frame f and point n: X = base[f?, n] + offsets[f, n] (the fp32 offset promoted, the sum
+ * in fp64; offsets may be NULL), t = (X, 1) . M_f^T, u = t . P, each dot product summed k = 0..3 with every operation
+ * rounded separately, then out[f, n] = (((u0 / u3) + 1) * 0.5 * width, ((u1 / u3) + 1) * 0.5 * height).
+ * offsets fp32 [L, N, 3] or NULL; base fp64 [N, 3] (base_per_frame = 0) or [L, N, 3] (1); matrices fp64 [L, 4, 4] row-major
+ * (device); proj: HOST array of 16 doubles, P row-major (u_j = sum_k t_k P[k][j]); out fp64 [L, N, 2].
+ */
+int ap_project_points_f64(const float* offsets, const double* base, int base_per_frame, const double* matrices,
+                          const double* proj, int L, int N, double width, double height, double* out, void* stream);
+
+/*
+ * Landmark pose frames, byte-identical to FaceMeshVisualizer.draw_landmarks (reference src/utils/draw_util.py:124-148:
+ * mediapipe drawing_utils.draw_landmarks with connections only, each edge a cv2.line(img, p0, p1, color, 2) in LINE_8 mode)
+ * on its 512 x 512 canvas, all L frames in one launch.
+ * keypoints fp64 [L, N, 2] (device). Landmark coordinates are the float32 values v = (float)(k / size) (size_x for x,
+ * size_y for y; normed != 0: v = (float)k); a landmark is kept iff 0 <= v <= 1 for both (NaN is dropped) and sits at pixel
+ * min(floor(v * 512), 511). edges int32 [E, 2] and colors uint8 [E, 3] are HOST arrays in draw order; an edge is drawn
+ * iff both landmarks are kept, later edges overwrite earlier ones, colour byte c goes to channel c.
+ * out: uint8 [L, 512, 512, 3], 16-byte aligned; 1 <= L <= AP_LMK_MAX_FRAMES (the 1-D grid has 32 CTAs per frame).
+ * Only thickness 2 and at most AP_LMK_MAX_EDGES edges are implemented; an
+ * edge index outside [0, N) is refused (AP_ERR_INVALID) before anything is launched. Deterministic.
+ */
+#define AP_LMK_CANVAS 512
+#define AP_LMK_MAX_EDGES 255
+#define AP_LMK_MAX_FRAMES 67108863
+int ap_draw_landmarks_u8(const double* keypoints, int L, int N, double size_x, double size_y, int normed,
+                         const int* edges, const unsigned char* colors, int E, int thickness, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
