@@ -74,4 +74,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     if (!(cond)) return ap::fail(AP_ERR_INVALID, __VA_ARGS__); \
   } while (0)
 
+// true for NULL and for any address on the 16-byte grid (the kernels' uint4 / float4 accesses need it)
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 }  // namespace ap

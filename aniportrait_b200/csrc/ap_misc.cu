@@ -630,6 +630,7 @@ extern "C" int ap_temporal_attention_f16(const void* qkv, long long ld, void* ou
 
 extern "C" int ap_add_f16(const void* a, const void* b, void* out, long long n, void* stream) {
   AP_REQUIRE(a && b && out && n % 8 == 0, "add: n must be a multiple of 8");
+  AP_REQUIRE(aligned16(a) && aligned16(b) && aligned16(out), "add: a, b and out must be 16-byte aligned");
   AP_LAUNCH((add_kernel), grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream, (const uint4*)a, (const uint4*)b, (uint4*)out, n / 8);
   AP_CHECK_CUDA(cudaGetLastError());
   return AP_OK;
@@ -637,6 +638,7 @@ extern "C" int ap_add_f16(const void* a, const void* b, void* out, long long n, 
 
 extern "C" int ap_add_bcast_f16(const void* a, const void* b, void* out, long long n, long long nb, void* stream) {
   AP_REQUIRE(a && b && out && n % 8 == 0 && nb % 8 == 0 && nb > 0 && n % nb == 0, "add_bcast: bad sizes");
+  AP_REQUIRE(aligned16(a) && aligned16(b) && aligned16(out), "add_bcast: a, b and out must be 16-byte aligned");
   AP_LAUNCH((add_bcast_kernel), grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream, (const uint4*)a, (const uint4*)b, (uint4*)out,
                                                                          n / 8, nb / 8);
   AP_CHECK_CUDA(cudaGetLastError());
@@ -660,6 +662,7 @@ extern "C" int ap_silu_f16(const void* x, void* out, long long n, void* stream) 
 
 extern "C" int ap_upsample2x_nhwc_f16(const void* x, void* out, int Nf, int H, int W, int C, void* stream) {
   AP_REQUIRE(x && out && C % 8 == 0, "upsample2x: C must be a multiple of 8");
+  AP_REQUIRE(aligned16(x) && aligned16(out), "upsample2x: x and out must be 16-byte aligned");
   const long long total = (long long)Nf * 4 * H * W * (C / 8);
   AP_LAUNCH((upsample2x_kernel), grid_for(total, 256), 256, 0, (cudaStream_t)stream, (const uint4*)x, (uint4*)out, Nf, H, W, C / 8);
   AP_CHECK_CUDA(cudaGetLastError());

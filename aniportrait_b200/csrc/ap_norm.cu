@@ -466,6 +466,7 @@ extern "C" int ap_groupnorm_nhwc_f16(const void* x, int C1, const void* x2, int 
   AP_REQUIRE(C1 % 8 == 0 && (!x2 || C2 % 8 == 0), "groupnorm: channel counts must be multiples of 8");
   AP_REQUIRE(C1 / 8 <= 1024 && (!x2 || C2 / 8 <= 1024), "groupnorm: too many channels");
   AP_REQUIRE(groups * 8 <= 1024, "groupnorm: at most 128 groups");
+  AP_REQUIRE(aligned16(x) && aligned16(x2) && aligned16(out), "groupnorm: x, x2 and out must be 16-byte aligned");
   const int cpg = C / groups;
   const int nsrc = x2 ? 2 : 1;
   const void* srcs[2] = {x, x2};
@@ -514,6 +515,7 @@ extern "C" int ap_groupnorm_apply_nhwc_f16(const void* x, int C1, const void* co
   AP_REQUIRE(C1 % 8 == 0 && (!x2 || C2 % 8 == 0), "groupnorm_apply: channel counts must be multiples of 8");
   AP_REQUIRE(HW % 32 == 0, "groupnorm_apply: HW=%d must be a multiple of 32 (32-row statistics entries)", HW);
   AP_REQUIRE(ld1 >= C1 && (!x2 || ld2 >= C2), "groupnorm_apply: partial row stride smaller than the channel count");
+  AP_REQUIRE(aligned16(x) && aligned16(x2) && aligned16(out), "groupnorm_apply: x, x2 and out must be 16-byte aligned");
   const int cpg = C / groups;
   float2* stat2 = reinterpret_cast<float2*>(stats);
   AP_LAUNCH((gn_finalize_cols_kernel), dim3(Nf, (groups + 7) / 8), 1024, 0, stream, 
@@ -563,6 +565,8 @@ extern "C" int ap_layernorm_f16(const void* x, long long rows, int C, float eps,
   AP_REQUIRE(x && out && gamma && beta, "layernorm: null pointer");
   AP_REQUIRE(C % 2 == 0 && C <= 64 * 32, "layernorm: C=%d unsupported (even, <= 2048)", C);
   AP_REQUIRE(pe == nullptr || (rows_per_pe > 0 && pe_period > 0), "layernorm: bad pe geometry");
+  AP_REQUIRE(aligned16(x) && aligned16(out) && aligned16(gamma) && aligned16(beta) && aligned16(pe),
+             "layernorm: x, out, gamma, beta and pe must be 16-byte aligned");
   const int wpb = 8;
   if (C % 8 == 0 && C / 8 <= 6 * 32 && getenv("AP_LAYERNORM_NARROW") == nullptr) {
     const int nvec = C / 8;

@@ -214,6 +214,7 @@ extern "C" int ap_batchnorm_train_nhwc_f16(const void* x, long long rows, int C,
   AP_REQUIRE(x && out && gamma && beta && workspace, "batchnorm: null pointer");
   AP_REQUIRE(act >= AP_ACT_NONE && act <= AP_ACT_GELU, "batchnorm: activation %d is not one of AP_ACT_*", act);
   AP_REQUIRE(rows > 0 && C > 0 && C % 8 == 0 && C / 8 <= 256, "batchnorm: C=%d must be a multiple of 8, <= 2048", C);
+  AP_REQUIRE(aligned16(x) && aligned16(out), "batchnorm: x and out must be 16-byte aligned");
   const int vecs = C / 8;
   int k = 256 / vecs;
   if (k < 1) k = 1;

@@ -107,6 +107,8 @@ int ap_conv3x3_nhwc_f16(const void* x, int C1, const void* x2, int C2, int Nf, i
  * x: [Nf, HW, C1], x2: [Nf, HW, C2] or NULL, out: [Nf, HW, C1+C2]; statistics per (frame, group) in fp32.
  * stats: caller-provided fp32 workspace of 2*groups*(Nf + 2*AP_GN_MAX_BLOCKS) floats ({mean, rstd} per (frame, group)
  * followed by per-block partial sums: the reduction is atomic-free, results are bit-reproducible run to run).
+ * x, x2 and out must be 16-byte aligned (16-byte loads and stores); C1, C2 multiples of 8. Nf * ceil(HW / rows per block)
+ * must fit AP_GN_MAX_BLOCKS (rows per block doubles up to HW to make it fit); otherwise AP_ERR_INVALID.
  */
 #define AP_GN_MAX_BLOCKS 2368
 int ap_groupnorm_nhwc_f16(const void* x, int C1, const void* x2, int C2, int Nf, int HW, int groups, float eps,
@@ -116,7 +118,7 @@ int ap_groupnorm_nhwc_f16(const void* x, int C1, const void* x2, int C2, int Nf,
  * The same GroupNorm with the statistics pass removed: {sum, sumsq} per channel and 32-row block were written by the
  * epilogue of the op that produced x (ap_epilogue_ext.col_stat_out of ap_gemm_f16 / ap_conv3x3_nhwc_f16); this call only
  * reduces them per (frame, group) and applies the normalisation. colstat*: fp32 pairs [Nf * HW / 32][ld*]; HW % 32 == 0,
- * at most 32 groups. stats: fp32 workspace of 2 * groups * Nf floats.
+ * at most 32 groups. stats: fp32 workspace of 2 * groups * Nf floats. x, x2 and out must be 16-byte aligned.
  */
 int ap_groupnorm_apply_nhwc_f16(const void* x, int C1, const void* colstat1, long long ld1, const void* x2, int C2,
                                 const void* colstat2, long long ld2, int Nf, int HW, int groups, float eps,
@@ -135,6 +137,8 @@ int ap_layernorm_finalize_f16(const void* row_stat, int parts, long long ld, lon
  * LayerNorm over the last dim (+ optional additive table pe[(row / rows_per_pe) % pe_period][C], the motion module's
  * sinusoidal frame encoding which the reference adds to the LayerNorm output, src/models/motion_module.py:365-366).
  * Replaces nn.LayerNorm (reference src/models/attention.py:331-362; src/models/motion_module.py:228-241).
+ * x/out [rows, C] fp16, C even and <= 2048; gamma, beta fp32 [C]; pe fp32 [pe_period, C] or NULL. x, out, gamma, beta and
+ * pe must be 16-byte aligned (also where C % 8 != 0 takes the 4-byte-access kernel: one contract for every width).
  */
 int ap_layernorm_f16(const void* x, long long rows, int C, float eps, const float* gamma, const float* beta,
                      const float* pe, int rows_per_pe, int pe_period, void* out, void* stream);
@@ -144,7 +148,7 @@ int ap_layernorm_f16(const void* x, long long rows, int C, float eps, const floa
  * activation `act` (AP_ACT_*; 1 keeps the former `relu` flag's meaning), channels-last. Replaces nn.BatchNorm2d + nn.ReLU
  * of the PoseGuider, which the reference never switches to eval mode (reference src/models/pose_guider.py:19-89;
  * scripts/pose2vid.py:102-110), and, with AP_ACT_GELU, wav2vec2's GroupNorm(512, 512) + GELU after its first convolution
- * (per-channel statistics over time for one clip). x/out: [rows, C] fp16, C % 8 == 0.
+ * (per-channel statistics over time for one clip). x/out: [rows, C] fp16, C % 8 == 0, both 16-byte aligned.
  * workspace: fp32, at least 2*C*(AP_BN_MAX_BLOCKS+1) floats (per-block partial sums, then the per-channel affine pair);
  * two-stage order-fixed reduction, double-precision finalize.
  */
@@ -286,7 +290,8 @@ int ap_attention_f16(const void* q, const void* k, const void* v, long long ld_q
 int ap_temporal_attention_f16(const void* qkv, long long ld, void* out, long long ldo, int B, int F, int N, int C,
                               int heads, float scale, void* stream);
 
-/* Elementwise / layout helpers (fp16, n % 8 == 0 where vectorised). */
+/* Elementwise / layout helpers (fp16, n % 8 == 0 where vectorised). ap_add_f16, ap_add_bcast_f16 and ap_upsample2x_nhwc_f16
+ * move 16-byte vectors: every pointer they take must be 16-byte aligned, or the call returns AP_ERR_INVALID. */
 int ap_add_f16(const void* a, const void* b, void* out, long long n, void* stream);          /* unet_3d.py:485-486,508-510 */
 int ap_silu_f16(const void* x, void* out, long long n, void* stream);                        /* resnet.py:226-230 */
 /* out[i] = a[i] + b[i % nb] (b broadcast over the leading CFG-branch dim) */
