@@ -752,6 +752,31 @@ def draw_landmarks(keypoints: torch.Tensor, size_x: float, size_y: float, normed
     return out
 
 
+RESIZE_MAX_SIDE = 8192   # AP_RESIZE_MAX_SIDE
+
+
+def resize_linear_u8(src: torch.Tensor, size, mid=None, out: torch.Tensor | None = None) -> torch.Tensor:
+    """cv2.resize(frame, size) (INTER_LINEAR) of every frame of uint8 src [L, h, w, 3] -> [L, H, W, 3] for size = (W, H),
+    in one launch (ap_resize_linear_u8). mid = (w', h'): cv2.resize(cv2.resize(frame, mid), size), the intermediate never
+    stored. out: a contiguous uint8 [L, H, W, 3] to write into instead of a new tensor."""
+    _ensure(src)
+    assert src.dtype == torch.uint8 and src.is_contiguous() and src.dim() == 4 and src.shape[3] == 3, (src.dtype, src.shape)
+    L, h, w, _ = src.shape
+    W, H = (int(v) for v in size)
+    mw, mh = (0, 0) if mid is None else (int(v) for v in mid)
+    for what, sides in (("source", (w, h)), ("intermediate", () if mid is None else (mw, mh)), ("output", (W, H))):
+        if not all(1 <= v <= RESIZE_MAX_SIDE for v in sides):   # refused before the output is allocated
+            raise ValueError(f"resize_linear_u8: {what} size {sides}: every side must lie in [1, {RESIZE_MAX_SIDE}]")
+    if out is None:
+        out = torch.empty(L, H, W, 3, dtype=torch.uint8, device=src.device)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (L, H, W, 3), (out.dtype, out.shape)
+    assert out.device == src.device
+    check(lib().ap_resize_linear_u8(ptr(src), I(L), I(w), I(h), I(mw), I(mh), I(W), I(H), ptr(out), stream_ptr()),
+          "ap_resize_linear_u8")
+    _count()
+    return out
+
+
 # --------------------------------------------------------------------------------------------------------------
 # Audio2Pose head-pose decoder
 # --------------------------------------------------------------------------------------------------------------

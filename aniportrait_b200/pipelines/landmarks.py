@@ -6,12 +6,15 @@ pose_util.project_points / project_points_with_trans (src/utils/pose_util.py:30-
     from aniportrait_b200.pipelines import landmarks
     vis = landmarks.enable_kernels(FaceMeshVisualizer(forehead_edge=False))
     kp = landmarks.project_points(pred, face_result["trans_mat"], pose_seq, [height, width], base=face_result["lmks3d"])
-    pose_frames = vis.draw_landmarks_batch((width, height), kp)       # CUDA uint8 [L, 512, 512, 3], one launch
+    pose_frames = vis.draw_pose_frames((width, height), kp)           # CUDA uint8 [L, height, width, 3]
     video = pipe(ref_image_pil, pose_frames, ref_pose, width, height, len(pose_frames), steps, cfg).videos
 
-The drawn bytes equal the reference's frame for frame. The host only builds the per-frame 4x4 matrices (the Euler angles
-to rotation restated in numpy, no scipy) and reads the edge table and colours from the caller's own visualizer; there is
-no CPU fallback.
+vid2vid draws at the source video's size and resizes once more (scripts/vid2vid.py:197-200):
+    pose_frames = vis.draw_pose_frames((frame_width, frame_height), kp, out_size=(width, height))
+
+The drawn bytes equal the reference's frame for frame, cv2.resize included. The host only builds the per-frame 4x4
+matrices (the Euler angles to rotation restated in numpy, no scipy) and reads the edge table and colours from the
+caller's own visualizer; there is no CPU fallback.
 """
 from __future__ import annotations
 
@@ -129,22 +132,64 @@ def edge_table(face_connection_spec):
 
 def _check_size(image_size):
     if tuple(int(v) for v in image_size) != (CANVAS, CANVAS):
-        raise NotImplementedError(f"draw_landmarks to image_size {tuple(image_size)}: the {CANVAS}x{CANVAS} canvas is "
-                                  "drawn exactly, the cv2.resize to any other size is not implemented")
+        raise NotImplementedError(f"draw_landmarks to image_size {tuple(image_size)}: draw_landmarks and "
+                                  f"draw_landmarks_batch draw the {CANVAS}x{CANVAS} canvas only; draw_pose_frames "
+                                  "draws at any size")
+
+
+def _frame_size(size, what):
+    """(W, H) as ints, each side in [1, ops.RESIZE_MAX_SIDE] (ValueError otherwise)."""
+    wh = tuple(int(v) for v in size)
+    if len(wh) != 2 or not all(1 <= v <= ops.RESIZE_MAX_SIDE for v in wh):
+        raise ValueError(f"{what} {tuple(size)}: expected (width, height), each in [1, {ops.RESIZE_MAX_SIDE}]")
+    return wh
+
+
+def resize_frames(frames, size) -> torch.Tensor:
+    """cv2.resize(frame, size) with the default INTER_LINEAR for every frame of CUDA uint8 frames [L, h, w, 3] ->
+    CUDA uint8 [L, H, W, 3] for size = (W, H), byte for byte, in one launch. Every side lies in [1, 8192]."""
+    if not (isinstance(frames, torch.Tensor) and frames.is_cuda and frames.dtype == torch.uint8):
+        raise TypeError("resize_frames takes a CUDA uint8 tensor [L, h, w, 3]")
+    if frames.dim() != 4 or frames.shape[3] != 3:
+        raise ValueError(f"frames must be [L, h, w, 3], got {tuple(frames.shape)}")
+    return ops.resize_linear_u8(frames.contiguous(), _frame_size(size, "size"))
+
+
+# frames drawn per launch by draw_pose_frames when it resizes: the 512 x 512 canvas scratch stays under 101 MB
+POSE_CHUNK = 128
+
+
+def _pose_stages(image_size, out_size):
+    """The sizes the canvas is resized to, in order: image_size (draw_landmarks' own cv2.resize), then out_size. A size
+    equal to the one before it is dropped: cv2.resize to the same size is a copy."""
+    sizes = [_frame_size(image_size, "image_size")]
+    if out_size is not None:
+        sizes.append(_frame_size(out_size, "out_size"))
+    stages, prev = [], (CANVAS, CANVAS)
+    for size in sizes:
+        if size != prev:
+            stages.append(size)
+        prev = size
+    return stages
 
 
 def enable_kernels(vis):
-    """Bind a FaceMeshVisualizer (reference src/utils/draw_util.py) to the device kernel. Its face_connection_spec is read
+    """Bind a FaceMeshVisualizer (reference src/utils/draw_util.py) to the device kernels. Its face_connection_spec is read
     once; afterwards
       vis.draw_landmarks(image_size, keypoints, normed=False)        -> numpy uint8 [H, W, 3], the reference's bytes
       vis.draw_landmarks_batch(image_size, keypoints, normed=False) -> CUDA uint8 [L, H, W, 3] for keypoints [L, N, C],
                                                                        one kernel launch, 1 <= L <= 67108863
+      vis.draw_pose_frames(image_size, keypoints, normed=False, out_size=None)
+          -> CUDA uint8 [L, H', W', 3]: per frame, cv2.resize(reference draw_landmarks(image_size, kp), out_size), or the
+             reference's draw_landmarks frame alone when out_size is None, at any sizes in [1, 8192]. Frames are drawn
+             in chunks of POSE_CHUNK, each one draw launch plus at most one resize launch (none when every resize is to
+             the size before it); no frame at image_size is stored when out_size differs from it.
     As in the reference, keypoints may carry more than two columns (LMKExtractor's [478, 3] x, y, z landmarks); only
-    columns 0 and 1 are read. Only image_size (512, 512) is implemented (NotImplementedError otherwise). Returns vis."""
+    columns 0 and 1 are read. draw_landmarks and draw_landmarks_batch implement image_size (512, 512) only
+    (NotImplementedError otherwise). Returns vis."""
     edges, colors = edge_table(vis.face_connection_spec)
 
-    def draw_landmarks_batch(image_size, keypoints, normed=False):
-        _check_size(image_size)
+    def device_keypoints(keypoints):
         if keypoints.ndim != 3 or keypoints.shape[2] < 2:
             raise ValueError(f"keypoints must be [L, N, C >= 2], got {tuple(keypoints.shape)}")
         n = keypoints.shape[1]
@@ -152,8 +197,26 @@ def enable_kernels(vis):
         if bad.any():
             a, b = edges[np.nonzero(bad.any(axis=1))[0][0]]
             raise ValueError(f"Landmark index is out of range. Invalid connection from landmark #{a} to landmark #{b}.")
-        kp = _to_device(keypoints[:, :, :2], torch.float64, _device(keypoints))
+        return _to_device(keypoints[:, :, :2], torch.float64, _device(keypoints))
+
+    def draw_landmarks_batch(image_size, keypoints, normed=False):
+        _check_size(image_size)
+        kp = device_keypoints(keypoints)
         return ops.draw_landmarks(kp, float(image_size[0]), float(image_size[1]), bool(normed), edges, colors)
+
+    def draw_pose_frames(image_size, keypoints, normed=False, out_size=None):
+        stages = _pose_stages(image_size, out_size)
+        kp = device_keypoints(keypoints)
+        size_x, size_y = float(image_size[0]), float(image_size[1])
+        if not stages:
+            return ops.draw_landmarks(kp, size_x, size_y, bool(normed), edges, colors)
+        W, H = stages[-1]
+        mid = stages[0] if len(stages) == 2 else None
+        out = torch.empty(kp.shape[0], H, W, 3, dtype=torch.uint8, device=kp.device)
+        for i in range(0, kp.shape[0], POSE_CHUNK):
+            canvas = ops.draw_landmarks(kp[i:i + POSE_CHUNK], size_x, size_y, bool(normed), edges, colors)
+            ops.resize_linear_u8(canvas, (W, H), mid=mid, out=out[i:i + POSE_CHUNK])
+        return out
 
     def draw_landmarks(image_size, keypoints, normed=False):
         if keypoints.ndim != 2:
@@ -162,4 +225,5 @@ def enable_kernels(vis):
 
     vis.draw_landmarks = draw_landmarks
     vis.draw_landmarks_batch = draw_landmarks_batch
+    vis.draw_pose_frames = draw_pose_frames
     return vis

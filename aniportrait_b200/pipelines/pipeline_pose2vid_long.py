@@ -177,8 +177,8 @@ class Pose2VideoPipeline:
         """cond_image_processor.preprocess for the pose maps. uint8 HxWx3 arrays of the target size (what the scripts
         pass, pose2vid.py:153-158) take a fast path: the bytes go to the GPU and the reference's `2*x - 1` (no /255, see
         image_processor.py) is evaluated there in fp32 — identical values, 4x fewer bytes over PCIe, no host float pass.
-        A CUDA uint8 tensor [L, height, width, 3] (the frames landmarks.enable_kernels(vis).draw_landmarks_batch draws on
-        the device) gives the same values with no host staging at all."""
+        A CUDA uint8 tensor [L, height, width, 3] (the frames landmarks.enable_kernels(vis).draw_landmarks_batch or
+        draw_pose_frames draws on the device) gives the same values with no host staging at all."""
         if (isinstance(pose_images, torch.Tensor) and pose_images.is_cuda and pose_images.dtype == torch.uint8
                 and pose_images.dim() == 4 and tuple(pose_images.shape[1:]) == (height, width, 3)):
             return pose_images.to(device).permute(0, 3, 1, 2).to(torch.float32) * 2.0 - 1.0

@@ -358,6 +358,20 @@ int ap_project_points_f64(const float* offsets, const double* base, int base_per
 int ap_draw_landmarks_u8(const double* keypoints, int L, int N, double size_x, double size_y, int normed,
                          const int* edges, const unsigned char* colors, int E, int thickness, void* out, void* stream);
 
+/*
+ * cv2.resize(frame, (dst_w, dst_h)) with the default INTER_LINEAR, byte-identical to OpenCV's 8-bit kernel (11-bit
+ * fixed-point coefficients, cv2's vectorised rounding of the vertical pass; a same-size resize is the identity and an exact
+ * 2x downscale equals cv2's INTER_AREA), for every frame: the resize FaceMeshVisualizer.draw_landmarks applies to its 512 x
+ * 512 canvas (reference src/utils/draw_util.py:146) and vid2vid's second one (scripts/vid2vid.py:199-200).
+ * src uint8 [L, src_h, src_w, 3] -> dst uint8 [L, dst_h, dst_w, 3] (device, contiguous).
+ * mid_w = mid_h = 0: one resize. Otherwise src -> (mid_w, mid_h) -> dst as two cv2.resize calls would give it; each mid pixel
+ * is recomputed from its source texels and rounded to uint8 as the stored image would be, and is never written to memory.
+ * Every side lies in [1, AP_RESIZE_MAX_SIDE]; anything else is refused (AP_ERR_INVALID) before a launch. Deterministic.
+ */
+#define AP_RESIZE_MAX_SIDE 8192
+int ap_resize_linear_u8(const void* src, int L, int src_w, int src_h, int mid_w, int mid_h, int dst_w, int dst_h,
+                        void* dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
