@@ -92,6 +92,12 @@ class PoseDecoderParams(ctypes.Structure):
                 ("cross", c_void_p)]
 
 
+class GridTile(ctypes.Structure):
+    """ap_grid_tile of include/aniportrait_b200.h."""
+    _fields_ = [("data", c_void_p), ("dtype", c_int), ("bgr", c_int), ("stride_t", c_longlong), ("stride_h", c_longlong),
+                ("stride_w", c_longlong), ("stride_c", c_longlong)]
+
+
 def ext_ptr(ext):
     """NULL or a pointer to an EpilogueExt (the struct is copied by the callee before it returns)."""
     if ext is None:

@@ -3,6 +3,7 @@
 
 #include "ap_host.h"
 #include "ap_ptx.cuh"
+#include "ap_u8.cuh"
 
 namespace ap {
 
@@ -516,14 +517,8 @@ __global__ void cfg_ddim_step_kernel(float* __restrict__ acc, const float* __res
 // Video frames -> packed 8-bit RGB (what the reference does on the host: src/utils/util.py:87-104 save_videos_grid,
 // `(x * 255).numpy().astype(np.uint8)` after an optional `(x + 1) / 2`, on the fp32 copy of the fp16 video). in: fp16
 // [B, 3, F, H, W] addressed through element strides (the decoder's frames live as [F, 3, H, W]); out: [B, F, H, W, 3]
-// bytes. Same fp32 operations in the same order as the host code (no fma contraction) -> bit-identical bytes; out-of-range
-// values saturate (the numpy cast is undefined there), NaN -> 0.
+// bytes. The per-sample arithmetic is ap_u8.cuh::to_u8.
 // ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned to_u8(__half h, int rescale) {
-  float x = __half2float(h);
-  if (rescale) x = __fmul_rn(__fadd_rn(x, 1.f), 0.5f);
-  return min(__float2uint_rz(__fmul_rn(x, 255.f)), 255u);   // cvt.rzi.u32.f32 saturates: negative and NaN -> 0
-}
 
 // VEC = 4: one thread packs four neighbouring pixels of a row (three 8-byte loads, three 4-byte stores); VEC = 1: any strides
 template <int VEC>

@@ -12,7 +12,7 @@ pids=()
 for src in *.cu; do
   obj=build/${src%.cu}.o
   objs+=("$obj")
-  if [[ ! -f "$obj" || "$src" -nt "$obj" || ap_ptx.cuh -nt "$obj" || ap_wgmma.cuh -nt "$obj" || ap_host.h -nt "$obj" || ../../include/aniportrait_b200.h -nt "$obj" ]]; then
+  if [[ ! -f "$obj" || "$src" -nt "$obj" || ap_ptx.cuh -nt "$obj" || ap_wgmma.cuh -nt "$obj" || ap_u8.cuh -nt "$obj" || ap_host.h -nt "$obj" || ../../include/aniportrait_b200.h -nt "$obj" ]]; then
     ( "$NVCC" "${FLAGS[@]}" -c "$src" -o "$obj" > "build/${src%.cu}.log" 2>&1 || { cat "build/${src%.cu}.log"; exit 1; } ) &
     pids+=($!)
   fi

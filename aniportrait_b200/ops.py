@@ -777,6 +777,98 @@ def resize_linear_u8(src: torch.Tensor, size, mid=None, out: torch.Tensor | None
     return out
 
 
+RESIZE_PIL_MAX_SCALE = 32   # AP_RESIZE_PIL_MAX_SCALE
+
+
+def resize_pil_bilinear_u8(src: torch.Tensor, size, out: torch.Tensor | None = None) -> torch.Tensor:
+    """Image.resize(size, Image.BILINEAR) (Pillow's 8-bit resampler) of every frame of uint8 RGB src [L, h, w, 3] ->
+    [L, H, W, 3] for size = (W, H), in one launch (ap_resize_pil_bilinear_u8); a same-size call is a device copy and no
+    launch. Every side lies in [1, RESIZE_MAX_SIDE] and no axis shrinks by more than RESIZE_PIL_MAX_SCALE. out: a contiguous
+    uint8 [L, H, W, 3] to write into instead of a new tensor."""
+    _ensure(src)
+    assert src.dtype == torch.uint8 and src.is_contiguous() and src.dim() == 4 and src.shape[3] == 3, (src.dtype, src.shape)
+    L, h, w, _ = src.shape
+    W, H = (int(v) for v in size)
+    for what, sides in (("source", (w, h)), ("output", (W, H))):
+        if not all(1 <= v <= RESIZE_MAX_SIDE for v in sides):   # refused before the output is allocated
+            raise ValueError(f"resize_pil_bilinear_u8: {what} size {sides}: every side must lie in [1, {RESIZE_MAX_SIDE}]")
+    if w > RESIZE_PIL_MAX_SCALE * W or h > RESIZE_PIL_MAX_SCALE * H:
+        raise ValueError(f"resize_pil_bilinear_u8: {(w, h)} -> {(W, H)} shrinks an axis by more than "
+                         f"{RESIZE_PIL_MAX_SCALE}x")
+    if out is None:
+        out = torch.empty(L, H, W, 3, dtype=torch.uint8, device=src.device)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (L, H, W, 3), (out.dtype, out.shape)
+    assert out.device == src.device
+    check(lib().ap_resize_pil_bilinear_u8(ptr(src), I(L), I(w), I(h), I(W), I(H), ptr(out), stream_ptr()),
+          "ap_resize_pil_bilinear_u8")
+    if (w, h) != (W, H):
+        _count()
+    return out
+
+
+GRID_MAX_TILES = 16   # AP_GRID_MAX_TILES
+_GRID_DTYPES = {torch.uint8: 0, torch.float16: 1, torch.float32: 2}   # AP_GRID_U8 / AP_GRID_F16 / AP_GRID_F32
+
+
+def grid_shape(B: int, n_rows: int, H: int, W: int):
+    """(GH, GW) of torchvision.utils.make_grid(padding=2) for B tiles of H x W; B = 1 is the tile itself."""
+    if B == 1:
+        return H, W
+    xmaps = min(n_rows, B)
+    return -(-B // xmaps) * (H + 2) + 2, xmaps * (W + 2) + 2
+
+
+def video_grid_u8(tiles, n_rows: int, T: int, bgr=None, out: torch.Tensor | None = None) -> torch.Tensor:
+    """save_videos_grid's frames of torch.cat(tiles) as uint8 [T, GH, GW, 3], in one launch (ap_video_grid_u8).
+    tiles: CUDA uint8 [T' >= T or 1, H, W, 3] frame bytes (T' = 1 repeats the frame; bgr[i] swaps their channels) or
+    fp16 / fp32 videos [1, 3, T' >= T, H, W] in [0, 1], any strides. out: a contiguous uint8 [T, GH, GW, 3] to reuse."""
+    B = len(tiles)
+    if not 1 <= B <= GRID_MAX_TILES:
+        raise ValueError(f"video_grid_u8: {B} tiles, expected 1 to {GRID_MAX_TILES}")
+    bgr = [False] * B if bgr is None else [bool(b) for b in bgr]
+    if len(bgr) != B:
+        raise ValueError(f"video_grid_u8: {len(bgr)} bgr flags for {B} tiles")
+    arr = (_lib.GridTile * B)()
+    H = W = None
+    for i, t in enumerate(tiles):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise TypeError(f"video_grid_u8: tile {i} is not a CUDA tensor (no CPU fallback)")
+        if t.dtype not in _GRID_DTYPES:
+            raise TypeError(f"video_grid_u8: tile {i} has dtype {t.dtype}; expected uint8, float16 or float32")
+        if t.dtype == torch.uint8:
+            if t.dim() != 4 or t.shape[3] != 3:
+                raise ValueError(f"video_grid_u8: uint8 tile {i} must be [T, H, W, 3], got {tuple(t.shape)}")
+            n, h, w = t.shape[:3]
+            st, sh, sw, sc = t.stride()
+        else:
+            if t.dim() != 5 or t.shape[0] != 1 or t.shape[1] != 3:
+                raise ValueError(f"video_grid_u8: video tile {i} must be [1, 3, T, H, W], got {tuple(t.shape)}")
+            if bgr[i]:
+                raise ValueError(f"video_grid_u8: the bgr flag applies to uint8 tiles only (tile {i})")
+            n, h, w = t.shape[2:]
+            _, sc, st, sh, sw = t.stride()
+        if n != 1 and n < T or (n == 1 and t.dtype != torch.uint8 and T > 1):
+            raise ValueError(f"video_grid_u8: tile {i} has {n} frames for a {T}-frame grid")
+        if (H, W) not in ((None, None), (h, w)):
+            raise ValueError(f"video_grid_u8: tile {i} is {h}x{w}, tile 0 is {H}x{W}")
+        H, W = h, w
+        if t.device != tiles[0].device:
+            raise ValueError(f"video_grid_u8: tile {i} is on {t.device}, tile 0 on {tiles[0].device}")
+        arr[i] = _lib.GridTile(t.data_ptr(), _GRID_DTYPES[t.dtype], int(bgr[i]), 0 if n == 1 else st, sh, sw, sc)
+    if T < 1 or n_rows < 1:
+        raise ValueError(f"video_grid_u8: T={T}, n_rows={n_rows}")
+    GH, GW = grid_shape(B, n_rows, H, W)
+    _ensure(tiles[0])
+    if out is None:
+        out = torch.empty(T, GH, GW, 3, dtype=torch.uint8, device=tiles[0].device)
+    if not (out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (T, GH, GW, 3)
+            and out.device == tiles[0].device):
+        raise ValueError(f"video_grid_u8: out must be a contiguous uint8 {(T, GH, GW, 3)} on {tiles[0].device}")
+    check(lib().ap_video_grid_u8(arr, I(B), I(n_rows), I(T), I(H), I(W), ptr(out), stream_ptr()), "ap_video_grid_u8")
+    _count()
+    return out
+
+
 # --------------------------------------------------------------------------------------------------------------
 # Audio2Pose head-pose decoder
 # --------------------------------------------------------------------------------------------------------------

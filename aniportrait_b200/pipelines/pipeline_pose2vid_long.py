@@ -708,9 +708,15 @@ class Pose2VideoPipeline:
         # "we always cast to float32" (reference :124-125): the conversion runs on the device and the result lands in ONE
         # pinned host buffer (a pageable fp16 copy + host-side conversion cost ~38 ms per 16-frame clip)
         # output_type="uint8" (not in the reference): packed RGB frames [B, F, H, W, 3] instead, see _to_host_u8
-        images = self._to_host_u8(video) if output_type == "uint8" else self._to_host_f32(video)
+        # output_type="cuda" (not in the reference): the decoded fp16 video [B, 3, F, H, W] in [0, 1] on the device, the
+        # tensor the host copies are made from (video_grid.grid_frames takes it as a tile)
+        if output_type == "cuda":
+            torch.cuda.current_stream(video.device).synchronize()      # collect_timings reads the run's events
+            images = video
+        else:
+            images = self._to_host_u8(video) if output_type == "uint8" else self._to_host_f32(video)
         self.collect_timings()
-        if output_type not in ("tensor", "uint8"):
+        if output_type not in ("tensor", "uint8", "cuda"):
             images = images.numpy()
         if not return_dict:
             return images

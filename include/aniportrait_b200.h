@@ -372,6 +372,51 @@ int ap_draw_landmarks_u8(const double* keypoints, int L, int N, double size_x, d
 int ap_resize_linear_u8(const void* src, int L, int src_w, int src_h, int mid_w, int mid_h, int dst_w, int dst_h,
                         void* dst, void* stream);
 
+/*
+ * Pillow's Image.resize((dst_w, dst_h), Image.BILINEAR) on RGB frames, byte-identical to its 8-bit resampler
+ * (libImaging/Resample.c: 22-bit fixed-point coefficients, horizontal pass first over the source rows the vertical pass
+ * reads, stored as uint8, then the vertical pass; a pass runs only where its axis changes size): what the scripts'
+ * transforms.Resize((height, width)) does to every frame shown beside the result (reference scripts/audio2vid.py:207-210,
+ * vid2vid.py:147-162, pose2vid.py:146-151). The coefficients are computed on the device in double with round-to-nearest
+ * intrinsics, as Pillow computes them.
+ * src uint8 [L, src_h, src_w, 3] -> dst uint8 [L, dst_h, dst_w, 3] (device, contiguous). Every side lies in
+ * [1, AP_RESIZE_MAX_SIDE] and each axis shrinks by at most AP_RESIZE_PIL_MAX_SCALE (src <= 32 * dst: up to 65 taps);
+ * anything else is refused (AP_ERR_INVALID) before a launch. Equal sizes are a device-to-device copy, no kernel.
+ * Deterministic.
+ */
+#define AP_RESIZE_PIL_MAX_SCALE 32
+int ap_resize_pil_bilinear_u8(const void* src, int L, int src_w, int src_h, int dst_w, int dst_h, void* dst,
+                              void* stream);
+
+/*
+ * The comparison grid the scripts save, in one launch: torch.cat of the tiles along the batch dim, then per frame
+ * torchvision.utils.make_grid(x, nrow=n_rows) (padding 2, pad value 0) and `(x * 255).numpy().astype(np.uint8)` as
+ * save_videos_grid does it (reference src/utils/util.py:87-104; scripts/audio2vid.py:245-260, vid2vid.py:228-243,
+ * pose2vid.py:181-196, app.py:258-262).
+ * out: uint8 [T, GH, GW, 3], GH = ymaps (H + 2) + 2, GW = xmaps (W + 2) + 2, xmaps = min(n_rows, B), ymaps = ceil(B / xmaps);
+ * tile i at (2 + (i / xmaps)(H + 2), 2 + (i % xmaps)(W + 2)); padding and unused cells 0. B = 1: the tile itself, [T, H, W, 3].
+ * tiles: HOST array of B descriptors, 1 <= B <= AP_GRID_MAX_TILES. Sample (t, y, x, c) of a tile is read at
+ *   data + t stride_t + y stride_h + x stride_w + c' stride_c (element strides; c' = 2 - c with bgr), for t < T:
+ *   AP_GRID_U8   uint8 bytes, written as they are (the ToTensor round trip trunc(fl(fl(v / 255) 255)) = v for every byte);
+ *                stride_t = 0 repeats frame 0 (the scripts' repeat of the reference image)
+ *   AP_GRID_F16  fp16 / AP_GRID_F32 fp32 values x in [0, 1]: trunc(fl(x * 255)) in fp32, saturated (ap_pack_frames_u8's bytes)
+ * The caller guarantees every tile has T frames (or stride_t = 0). Deterministic.
+ */
+#define AP_GRID_U8 0
+#define AP_GRID_F16 1
+#define AP_GRID_F32 2
+#define AP_GRID_MAX_TILES 16
+typedef struct ap_grid_tile {
+  const void* data;
+  int dtype;
+  int bgr;
+  long long stride_t;
+  long long stride_h;
+  long long stride_w;
+  long long stride_c;
+} ap_grid_tile;
+int ap_video_grid_u8(const ap_grid_tile* tiles, int B, int n_rows, int T, int H, int W, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
