@@ -83,7 +83,8 @@ class EpilogueExt(ctypes.Structure):
 
 
 class PoseDecoderParams(ctypes.Structure):
-    """ap_pose_decoder_params of include/aniportrait_b200.h."""
+    """ap_pose_decoder_params of include/aniportrait_b200.h, taken by ap_pose_decoder_f16 and by its test hook
+    ap_pose_decoder_trace_f16(params, T, kv_cache, out, trace, stream), which also writes every stage's input."""
     _fields_ = [("layers", c_int), ("out_dim", c_int), ("embed_dim", c_int), ("heads", c_int), ("ffn_dim", c_int),
                 ("mask_len", c_int), ("pe_len", c_int), ("eps", c_float),
                 ("w_qkv", c_void_p), ("w_out", c_void_p), ("w_ff1", c_void_p), ("w_ff2", c_void_p), ("vec", c_void_p),

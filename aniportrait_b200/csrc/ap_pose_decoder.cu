@@ -27,6 +27,9 @@
 // Numerics: fp16 weights and KV cache; everything else fp32 (activations, accumulation, LayerNorm statistics, softmax,
 // biases, cross, pe, mask, pose head, output). Every reduction has a fixed order and there are no atomics: two calls give
 // identical bytes.
+#include <cstdlib>
+#include <cstring>
+
 #include "ap_host.h"
 #include "ap_ptx.cuh"
 
@@ -262,9 +265,24 @@ struct PoseArgs {
   int T;
   float* out;
   __half* kv;
+  float* trace;   // pose_decoder_kernel<NC, true> only: fp32 [T, PD_TRACE_STAGES * layers + 1, 512]
 };
 
-template <int NC>
+// With TRACE, the kernel stores the input of every stage of every layer, so that a test can check each stage on its own
+// inputs: row (i, 5 l + k) of step i, layer l holds k = 0 the layer input x, 1 q, 2 the attention output of all heads,
+// 3 the LN2 output (linear1's input), 4 linear2 + bias + residual (LN3's input); row (i, 5 layers) the pose head's input.
+// The vectors are identical in every CTA, so CTA 0 stores them; q lives in the head owner's CTA (h < 8), which stores
+// its 64 entries. `if constexpr` keeps the production instantiations free of it: the 16-CTA kernel sits at the
+// 128-register cap.
+constexpr int PD_TRACE_STAGES = 5;
+template <bool TRACE>
+__device__ __forceinline__ void trace_store(const PoseArgs& a, bool who, int i, int row, int e, float v) {
+  if constexpr (TRACE) {
+    if (who) a.trace[((size_t)i * (PD_TRACE_STAGES * a.p.layers + 1) + row) * PD_E + e] = v;
+  }
+}
+
+template <int NC, bool TRACE>
 __global__ void __launch_bounds__(PD_THREADS, 1) pose_decoder_kernel(const PoseArgs args) {
   using S = PoseShape<NC>;
   griddep_launch_dependents();   // PDL: see ap_host.h::launch_pdl
@@ -320,6 +338,7 @@ __global__ void __launch_bounds__(PD_THREADS, 1) pose_decoder_kernel(const PoseA
         const float* pp = pbuf + ((g - 1) & 1) * S::PFLOATS;
         xs[tid] = layer_norm(hs[tid], pp + 4 * PD_E, pp + 5 * PD_E, p.eps, br);
       }
+      trace_store<TRACE>(args, rank == 0, i, PD_TRACE_STAGES * l, tid, xs[tid]);
       __syncthreads();
       // the block of layer g - 1 has been read for the last time (its LN3 ran above, or at the end of the last step)
       if (tid == 0 && g >= 1) st.issue_params(g + 1, pbuf, pbar, T);
@@ -344,6 +363,8 @@ __global__ void __launch_bounds__(PD_THREADS, 1) pose_decoder_kernel(const PoseA
           const int which = 1 + tid / PD_D, d = tid % PD_D;
           (which == 1 ? kc : vc)[(size_t)i * PD_D + d] = __float2half_rn(qkv[which][d]);
         }
+        trace_store<TRACE>(args, tid < PD_D, i, PD_TRACE_STAGES * l + 1, h * PD_D + (tid & (PD_D - 1)),
+                           qkv[0][tid & (PD_D - 1)]);
         __syncthreads();
         const float* mrow = p.mask + ((size_t)h * p.mask_len + i) * p.mask_len;
         float m = -INFINITY;
@@ -406,6 +427,7 @@ __global__ void __launch_bounds__(PD_THREADS, 1) pose_decoder_kernel(const PoseA
       }
       cluster_arrive();
       cluster_wait();
+      trace_store<TRACE>(args, rank == 0, i, PD_TRACE_STAGES * l + 2, tid, as_[tid]);
       // ---- C: out_proj rows + bias + residual
       gemv_phase<PD_E, S::NCo>(as_, ring, full, q, st, [&](int r, float o) {
         const int row = (int)rank * S::BO + r;
@@ -419,6 +441,7 @@ __global__ void __launch_bounds__(PD_THREADS, 1) pose_decoder_kernel(const PoseA
         float y = layer_norm(hs[tid], pp + 0 * PD_E, pp + 1 * PD_E, p.eps, br);
         y = y + pp[S::P_CR + tid];
         xs[tid] = layer_norm(y, pp + 2 * PD_E, pp + 3 * PD_E, p.eps, br);
+        trace_store<TRACE>(args, rank == 0, i, PD_TRACE_STAGES * l + 3, tid, xs[tid]);
         __syncthreads();
         gemv_phase<PD_E, S::ND>(xs, ring, full, q, st, [&](int r, float o) {
           const int row = (int)rank * S::B1 + r;
@@ -436,12 +459,14 @@ __global__ void __launch_bounds__(PD_THREADS, 1) pose_decoder_kernel(const PoseA
       });
       cluster_arrive();
       cluster_wait();
+      trace_store<TRACE>(args, rank == 0, i, PD_TRACE_STAGES * l + 4, tid, hs[tid]);
     }
     // ---- pose head and next token, redundantly in every CTA (no remote stores: hs is not written again before the next
     // step's phase C, two barriers away)
     {
       const float* pp = pbuf + (((long long)i * L + L - 1) & 1) * S::PFLOATS;
       xs[tid] = layer_norm(hs[tid], pp + 4 * PD_E, pp + 5 * PD_E, p.eps, br);
+      trace_store<TRACE>(args, rank == 0, i, PD_TRACE_STAGES * L, tid, xs[tid]);
       __syncthreads();
       if (warp < od) {
         float s = 0.f;
@@ -466,18 +491,23 @@ __global__ void __launch_bounds__(PD_THREADS, 1) pose_decoder_kernel(const PoseA
 }
 
 // Cluster size per device, chosen once: 16 CTAs if the device can co-schedule a cluster of 16 with this kernel's resources
-// (a non-portable size), else 8; 0 = not chosen yet, < 0 = neither can run.
+// (a non-portable size), else 8; AP_POSE_CTAS=8|16 asks for one size instead (both sizes compute identical bytes; the
+// override lets one device test the 8-CTA kernel). 0 = not chosen yet, < 0 = minus the size that cannot run.
 constexpr int PD_MAX_DEVICES = 64;
 static int g_pose_ctas[PD_MAX_DEVICES] = {0};
 
+template <int NC, bool TRACE>
+static bool allow_cluster_smem() {   // the non-portable cluster size and the dynamic shared memory of one instantiation
+  if (NC > 8 && cudaFuncSetAttribute(pose_decoder_kernel<NC, TRACE>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) !=
+                    cudaSuccess)
+    return false;
+  return cudaFuncSetAttribute(pose_decoder_kernel<NC, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)PoseShape<NC>::SMEM) == cudaSuccess;
+}
+
 template <int NC>
 static int max_active_clusters() {
-  if (NC > 8 && cudaFuncSetAttribute(pose_decoder_kernel<NC>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) !=
-                    cudaSuccess)
-    return 0;
-  if (cudaFuncSetAttribute(pose_decoder_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                           (int)PoseShape<NC>::SMEM) != cudaSuccess)
-    return 0;
+  if (!allow_cluster_smem<NC, false>()) return 0;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(NC);
   cfg.blockDim = dim3(PD_THREADS);
@@ -490,7 +520,7 @@ static int max_active_clusters() {
   cfg.attrs = &attr;
   cfg.numAttrs = 1;
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, pose_decoder_kernel<NC>, &cfg) != cudaSuccess) n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, pose_decoder_kernel<NC, false>, &cfg) != cudaSuccess) n = 0;
   return n;
 }
 
@@ -499,24 +529,35 @@ static int pose_ctas(int* out) {
   AP_CHECK_CUDA(cudaGetDevice(&dev));
   AP_REQUIRE(dev >= 0 && dev < PD_MAX_DEVICES, "pose_decoder: device %d out of range", dev);
   if (g_pose_ctas[dev] == 0) {
-    g_pose_ctas[dev] = max_active_clusters<16>() > 0 ? 16 : (max_active_clusters<8>() > 0 ? 8 : -1);
+    const char* want = getenv("AP_POSE_CTAS");
+    AP_REQUIRE(!want || !strcmp(want, "8") || !strcmp(want, "16"), "pose_decoder: AP_POSE_CTAS=%s must be 8 or 16", want);
+    if (want && !strcmp(want, "8"))
+      g_pose_ctas[dev] = max_active_clusters<8>() > 0 ? 8 : -8;
+    else if (want)
+      g_pose_ctas[dev] = max_active_clusters<16>() > 0 ? 16 : -16;
+    else
+      g_pose_ctas[dev] = max_active_clusters<16>() > 0 ? 16 : (max_active_clusters<8>() > 0 ? 8 : -8);
     cudaGetLastError();   // a refused query must not leave an error behind for the next launch
   }
-  if (g_pose_ctas[dev] < 0) return fail(AP_ERR_CUDA, "pose_decoder: the device cannot co-schedule a cluster of 8 CTAs");
+  if (g_pose_ctas[dev] < 0)
+    return fail(AP_ERR_CUDA, "pose_decoder: the device cannot co-schedule a cluster of %d CTAs", -g_pose_ctas[dev]);
   *out = g_pose_ctas[dev];
   return AP_OK;
 }
 
-}  // namespace ap
-
-using namespace ap;
-
-extern "C" int ap_pose_decoder_ctas(int* ctas) {
-  AP_REQUIRE(ctas, "pose_decoder_ctas: null pointer");
-  return pose_ctas(ctas);
+template <int NC, bool TRACE>
+static cudaError_t launch_decoder(const PoseArgs& args, void* stream) {
+  if (TRACE && !allow_cluster_smem<NC, TRACE>()) {   // the test hook sets its own attributes, at its own launches
+    const cudaError_t e = cudaGetLastError();
+    return e != cudaSuccess ? e : cudaErrorInvalidConfiguration;
+  }
+  return launch_pdl(pose_decoder_kernel<NC, TRACE>, dim3(NC), dim3(PD_THREADS), PoseShape<NC>::SMEM,
+                    (cudaStream_t)stream, NC, args);
 }
 
-extern "C" int ap_pose_decoder_f16(const ap_pose_decoder_params* params, int T, void* kv_cache, float* out, void* stream) {
+// ap_pose_decoder_f16 (trace == nullptr) and its traced test hook: one validation, one launch.
+static int pose_decoder(const ap_pose_decoder_params* params, int T, void* kv_cache, float* out, float* trace,
+                        void* stream) {
   AP_REQUIRE(params && kv_cache && out, "pose_decoder: null pointer");
   const ap_pose_decoder_params& p = *params;
   AP_REQUIRE(p.w_qkv && p.w_out && p.w_ff1 && p.w_ff2 && p.vec && p.pose_map_w && p.pose_map_b && p.pose_map_r_w &&
@@ -533,18 +574,36 @@ extern "C" int ap_pose_decoder_f16(const ap_pose_decoder_params* params, int T, 
   const void* a16[] = {p.w_qkv, p.w_out, p.w_ff1, p.w_ff2, p.vec, p.cross, kv_cache};
   for (const void* q : a16) AP_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15) == 0, "pose_decoder: the weights, vec, cross "
                                        "and the KV cache must be 16-byte aligned");
-  const float* a4[] = {p.pose_map_w, p.pose_map_b, p.pose_map_r_w, p.pose_map_r_b, p.pe, p.id_row, p.mask, out};
+  const float* a4[] = {p.pose_map_w, p.pose_map_b, p.pose_map_r_w, p.pose_map_r_b, p.pe, p.id_row, p.mask, out, trace};
   for (const float* q : a4) AP_REQUIRE((reinterpret_cast<uintptr_t>(q) & 3) == 0, "pose_decoder: fp32 operands must be "
                                        "4-byte aligned");
   int nc = 0;
   int rc = pose_ctas(&nc);
   if (rc) return rc;
-  PoseArgs args{p, T, out, reinterpret_cast<__half*>(kv_cache)};
-  cudaError_t e = nc == 16 ? launch_pdl(pose_decoder_kernel<16>, dim3(16), dim3(PD_THREADS), PoseShape<16>::SMEM,
-                                        (cudaStream_t)stream, 16, args)
-                           : launch_pdl(pose_decoder_kernel<8>, dim3(8), dim3(PD_THREADS), PoseShape<8>::SMEM,
-                                        (cudaStream_t)stream, 8, args);
-  if (e != cudaSuccess) return fail(AP_ERR_CUDA, "launch pose_decoder_kernel<%d>: %s", nc, cudaGetErrorString(e));
+  PoseArgs args{p, T, out, reinterpret_cast<__half*>(kv_cache), trace};
+  cudaError_t e = nc == 16 ? (trace ? launch_decoder<16, true>(args, stream) : launch_decoder<16, false>(args, stream))
+                           : (trace ? launch_decoder<8, true>(args, stream) : launch_decoder<8, false>(args, stream));
+  if (e != cudaSuccess)
+    return fail(AP_ERR_CUDA, "launch pose_decoder_kernel<%d%s>: %s", nc, trace ? ", trace" : "", cudaGetErrorString(e));
   AP_CHECK_CUDA(cudaGetLastError());
   return AP_OK;
+}
+
+}  // namespace ap
+
+using namespace ap;
+
+extern "C" int ap_pose_decoder_ctas(int* ctas) {
+  AP_REQUIRE(ctas, "pose_decoder_ctas: null pointer");
+  return pose_ctas(ctas);
+}
+
+extern "C" int ap_pose_decoder_f16(const ap_pose_decoder_params* params, int T, void* kv_cache, float* out, void* stream) {
+  return pose_decoder(params, T, kv_cache, out, nullptr, stream);
+}
+
+extern "C" int ap_pose_decoder_trace_f16(const ap_pose_decoder_params* params, int T, void* kv_cache, float* out,
+                                         float* trace, void* stream) {
+  AP_REQUIRE(trace, "pose_decoder_trace: null trace pointer");
+  return pose_decoder(params, T, kv_cache, out, trace, stream);
 }

@@ -223,7 +223,13 @@ int ap_patchify_nchw_f16(const void* pixels, int in_f32, int B, int H, int W, in
  * Numerics: fp16 weights and KV cache, fp32 everything else; fixed reduction order, no atomics (bit-reproducible).
  * The grid is one thread-block cluster of 16 CTAs (8 where the device cannot co-schedule 16), one SM each (about 222 KB of
  * shared memory per CTA), chosen once per device at the first call; ap_pose_decoder_ctas reports the choice (and makes it
- * if not made yet).
+ * if not made yet). AP_POSE_CTAS=8 or 16 in the environment at that first call asks for that size instead (both sizes
+ * give identical bytes): AP_ERR_CUDA if the device cannot co-schedule it, AP_ERR_INVALID for any other value.
+ * ap_pose_decoder_trace_f16 is a test hook with the same contract that also writes the input of every stage into trace
+ * fp32 [T, 5 * layers + 1, 512] (4-byte aligned): row (i, 5 l + k) of step i, layer l holds k = 0 the layer input x
+ * (row (i, 0) = token + (pe[i] + id_row)), 1 q (in_proj + bias), 2 the attention output of the 8 heads, 3 the LN2
+ * output, 4 x2 + linear2(relu(linear1(x2))) before LN3; row (i, 5 layers) the input of pose_map_r. Its out and kv_cache
+ * equal those of ap_pose_decoder_f16 bit for bit.
  */
 #define AP_POSE_VEC 6656
 #define AP_POSE_B_QKV 0
@@ -260,6 +266,8 @@ typedef struct ap_pose_decoder_params {
   const float* cross;
 } ap_pose_decoder_params;
 int ap_pose_decoder_f16(const ap_pose_decoder_params* params, int T, void* kv_cache, float* out, void* stream);
+int ap_pose_decoder_trace_f16(const ap_pose_decoder_params* params, int T, void* kv_cache, float* out, float* trace,
+                              void* stream);
 int ap_pose_decoder_ctas(int* ctas);
 
 /* Row softmax, fp16 in/out (may be in place), fp32 math: the VAE mid-block attention (single head, d = 512) is evaluated as
