@@ -483,7 +483,9 @@ __global__ void scatter_accumulate_kernel(const __half* __restrict__ pred, int l
   *d = a;
 }
 
-// noise = acc / count ; CFG: u + g (c - u) ; DDIM v-prediction step (eta = 0) ; latents updated in place; acc zeroed.
+// noise = acc * inv_count ; CFG: u + g (c - u) ; DDIM step (eta = 0) ; latents updated in place; acc zeroed.
+// inv_count is the caller's per-frame weight: 1 / count under CFG (the overlap average), 1 without CFG, where the reference
+// steps on the sum of the overlapping windows' predictions (pipeline_pose2vid_long.py:551-559; sharding.step_weights).
 // x0 = c_xx x + c_xv v, eps = c_ex x + c_ev v (the three diffusers prediction types differ only in these coefficients),
 // optional clamp of x0 (clip_sample; eps is NOT recomputed: use_clipped_model_output = False), then the eta = 0 update.
 __global__ void cfg_ddim_step_kernel(float* __restrict__ acc, const float* __restrict__ inv_count, int cfg, float guidance,
@@ -683,6 +685,10 @@ extern "C" int ap_nhwc_to_ncfhw_f16(const void* x, void* out, int B, int C, int 
 extern "C" int ap_gather_window_f16(const void* latents, const int* frame_idx, void* out, int dup, int F, int HW,
                                     int Cpad, void* stream) {
   AP_REQUIRE(latents && frame_idx && out && Cpad % 8 == 0 && Cpad >= 8, "gather_window: bad arguments");
+  AP_REQUIRE(dup >= 1 && F >= 1 && HW >= 1, "gather_window: dup=%d F=%d HW=%d must be positive", dup, F, HW);
+  // the kernel loads a pixel's 4 latent channels as one uint2 and stores Cpad-channel rows as uint4
+  AP_REQUIRE((reinterpret_cast<uintptr_t>(latents) & 7) == 0 && aligned16(out),
+             "gather_window: latents must be 8-byte and out 16-byte aligned");
   const long long total = (long long)dup * F * HW;
   AP_LAUNCH((gather_window_kernel), (unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream, 
       (const __half*)latents, frame_idx, (__half*)out, dup, F, HW, Cpad);
@@ -693,6 +699,10 @@ extern "C" int ap_gather_window_f16(const void* latents, const int* frame_idx, v
 extern "C" int ap_scatter_accumulate_f16(const void* pred, int ld, const int* frame_idx, float* acc, int B, int F,
                                          int L, int HW, void* stream) {
   AP_REQUIRE(pred && frame_idx && acc, "scatter_accumulate: null pointer");
+  AP_REQUIRE(B >= 1 && F >= 1 && L >= 1 && HW >= 1 && ld >= 4,
+             "scatter_accumulate: B=%d F=%d L=%d HW=%d must be positive and ld=%d >= 4", B, F, L, HW, ld);
+  // one float4 read-modify-write per (b, frame, pixel)
+  AP_REQUIRE(aligned16(acc), "scatter_accumulate: acc must be 16-byte aligned");
   const long long total = (long long)B * F * HW;
   AP_LAUNCH((scatter_accumulate_kernel), (unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream, 
       (const __half*)pred, ld, frame_idx, acc, B, F, L, HW);
@@ -704,6 +714,7 @@ extern "C" int ap_cfg_ddim_step_f16(float* acc, const float* inv_count, int cfg,
                                     float alpha_prev, int prediction_type, float clip_range, void* latents, int L, int HW,
                                     void* stream) {
   AP_REQUIRE(acc && inv_count && latents, "cfg_ddim_step: null pointer");
+  AP_REQUIRE(L >= 1 && HW >= 1, "cfg_ddim_step: L=%d HW=%d must be positive", L, HW);
   const float sa = sqrtf(alpha_t), sb = sqrtf(1.f - alpha_t);
   float c_xx, c_xv, c_ex, c_ev;
   if (prediction_type == AP_PRED_V) {

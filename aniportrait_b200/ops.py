@@ -670,8 +670,10 @@ PREDICTION_TYPES = {"v_prediction": 0, "epsilon": 1, "sample": 2}   # AP_PRED_* 
 
 def cfg_ddim_step(acc: torch.Tensor, inv_count: torch.Tensor, guidance: float, alpha_t: float, alpha_prev: float,
                   latents: torch.Tensor, prediction_type: str = "v_prediction", clip_range: float = 0.0):
-    """In place: latents <- DDIM (eta = 0) step of the CFG-combined, overlap-averaged prediction; acc zeroed.
-    clip_range > 0 clamps the predicted x0 (DDIMScheduler clip_sample)."""
+    """In place: latents <- DDIM (eta = 0) step of the CFG-combined prediction acc * inv_count; acc zeroed.
+    inv_count holds per-frame weights: 1 / count (the overlap average) under CFG, 1 without CFG, where the reference steps
+    on the sum of the windows' predictions (sharding.step_weights). clip_range > 0 clamps the predicted x0
+    (DDIMScheduler clip_sample)."""
     if prediction_type not in PREDICTION_TYPES:
         raise ValueError(f"prediction_type {prediction_type!r} is not one of {sorted(PREDICTION_TYPES)}")
     _ensure(latents)

@@ -27,7 +27,7 @@ import torch
 from .. import ops
 from ..models.clip_vision import kernels_enabled
 from ..models.mutual_self_attention import ReferenceAttentionControl
-from .sharding import plan_units, plan_windows, windows_of_rank
+from .sharding import plan_units, plan_windows, step_weights, windows_of_rank
 from .image_processor import VaeImageProcessor
 
 
@@ -549,7 +549,7 @@ class Pose2VideoPipeline:
         else:
             my_windows = windows_of_rank(windows, rank, world, shard)
             units = [(k, "both") for k in range(len(my_windows))]
-        inv_count = inv_count.to(device=device, dtype=torch.float32)
+        inv_count = step_weights(inv_count, cfg).to(device=device, dtype=torch.float32)
         clip_is_embed = clip_image_embeds is not None
         clip_in = clip_image_embeds if clip_is_embed else clip_pixels
         static = bool(self.use_cuda_graph)

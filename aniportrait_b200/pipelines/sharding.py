@@ -1,8 +1,9 @@
 """Host-side work partitioning of the denoising loop (SURVEY.md §8e). Pure Python / CPU torch: unit-testable with gloo.
 
 Within one DDIM step every context window is an independent UNet call (reference pipeline_pose2vid_long.py:519-548);
-their predictions are summed per frame, divided by the per-frame window count, CFG-combined and stepped. Sharding the
-windows over ranks therefore needs exactly one sum-all-reduce of the fp32 accumulator per step."""
+their predictions are summed per frame; under CFG the sums are divided by the per-frame window count and CFG-combined,
+without CFG the reference steps on the sums themselves (:551-559). Sharding the windows over ranks therefore needs
+exactly one sum-all-reduce of the fp32 accumulator per step."""
 from __future__ import annotations
 
 from typing import List
@@ -70,10 +71,18 @@ def accumulate(acc: torch.Tensor, pred: torch.Tensor, window: List[int]):
     return acc
 
 
+def step_weights(inv_count: torch.Tensor, cfg: bool) -> torch.Tensor:
+    """Per-frame weights of the accumulated predictions that ap_cfg_ddim_step_f16 takes as its inv_count. The reference
+    divides by the window count only under CFG (:551-552: `noise_pred / counter` sits inside `if
+    do_classifier_free_guidance`); without CFG it steps on the sum of the overlapping windows' predictions."""
+    return inv_count if cfg else torch.ones_like(inv_count)
+
+
 def combine(acc: torch.Tensor, inv_count: torch.Tensor, guidance: float):
-    """Overlap average + classifier-free guidance (reference :551-555). acc [B, L, ...] -> [L, ...]."""
+    """The prediction the reference steps on (:551-557). acc [B, L, ...] -> [L, ...]: B == 2 (CFG) is the overlap average
+    then classifier-free guidance, B == 1 the plain sum over the windows."""
     shape = [1, -1] + [1] * (acc.dim() - 2)
-    avg = acc * inv_count.view(*shape)
+    avg = acc * step_weights(inv_count, acc.shape[0] == 2).view(*shape)
     if acc.shape[0] == 2:
         return avg[0] + guidance * (avg[1] - avg[0])
     return avg[0]

@@ -313,9 +313,13 @@ int ap_nhwc_to_ncfhw_f16(const void* x, void* out, int B, int C, int F, int HW, 
 /*
  * Denoising-loop elementwise ops (reference src/pipelines/pipeline_pose2vid_long.py:521-559 and diffusers
  * DDIMScheduler.step [dep], eta = 0). latents: fp16 [L, HW, 4] channels-last; acc: fp32 [B, L, HW, 4].
- * ap_cfg_ddim_step_f16: overlap average + classifier-free guidance + one DDIM update, in place on `latents`; `acc` is
- * zeroed. prediction_type: AP_PRED_* (configs/inference/inference_v2.yaml:30 uses v_prediction, inference_v1.yaml
- * epsilon); clip_range > 0 clamps the predicted x0 to [-clip_range, clip_range] (DDIMScheduler clip_sample), <= 0: off.
+ * ap_gather_window_f16: `latents` 8-byte and `out` 16-byte aligned; dup, F, HW >= 1.
+ * ap_scatter_accumulate_f16: `acc` 16-byte aligned; B, F, L, HW >= 1 and ld >= 4. Otherwise AP_ERR_INVALID, no launch.
+ * ap_cfg_ddim_step_f16: per-frame weighting (acc * inv_count) + classifier-free guidance + one DDIM update, in place on
+ * `latents`; `acc` is zeroed. inv_count is 1 / count for the overlap average the reference takes under CFG, and 1
+ * without CFG, where the reference steps on the sum of the windows' predictions. prediction_type: AP_PRED_*
+ * (configs/inference/inference_v2.yaml:30 uses v_prediction, inference_v1.yaml epsilon); clip_range > 0 clamps the
+ * predicted x0 to [-clip_range, clip_range] (DDIMScheduler clip_sample), <= 0: off.
  */
 #define AP_PRED_V 0
 #define AP_PRED_EPSILON 1

@@ -351,6 +351,9 @@ CASES = {
     "host_logic": case_host_logic,
     "oracle_reference_small": case_oracle_pins,
     "pipeline_small": case_pipeline,
+    # the same run without CFG (guidance 1.0): the reference steps on the SUM of the overlapping windows' predictions
+    # (pipeline_pose2vid_long.py:551-552 divide by the counter only under CFG); 12 of the 20 frames lie in both windows
+    "pipeline_small_no_cfg": lambda: case_pipeline("pipeline_small_no_cfg", dict(PIPE_SMALL, guidance=1.0)),
     "pipeline_c1_full": case_pipeline_c1,
     # the benchmarked geometry (BASELINE.json configs[1]): full width, 64x64 latents, one 16-frame window under CFG
     "unet3d_full_f16_64x64": lambda: case_unet3d("unet3d_full_f16_64x64", (320, 640, 1280, 1280), 16, 64, 64, 479,

@@ -174,6 +174,33 @@ def test_window_sharding_world2_gloo():
     assert torch.allclose(torch.from_numpy(got), ref, atol=1e-5)
 
 
+def test_step_weights_and_combine_follow_the_reference_with_and_without_cfg():
+    """The reference (pipeline_pose2vid_long.py:546-557) divides the window sums by the counter only under CFG; without
+    CFG it steps on the sum. step_weights gives ap_cfg_ddim_step_f16 weights 1 / count or 1, and combine matches."""
+    from aniportrait_b200.pipelines.sharding import accumulate, combine, plan_windows, step_weights
+    L = 20
+    windows, inv = plan_windows(L, 25)
+    assert len(windows) == 2 and int((inv < 1).sum()) == 12
+    assert torch.equal(step_weights(inv, True), inv)
+    assert torch.equal(step_weights(inv, False), torch.ones(L))
+    g = torch.Generator().manual_seed(1)
+    for cfg in (False, True):
+        B = 2 if cfg else 1
+        noise = torch.zeros(B, 4, L, 3, 3, dtype=torch.float64)      # the reference's layout and loop
+        counter = torch.zeros(1, 1, L, 1, 1, dtype=torch.float64)
+        acc = torch.zeros(B, L, 4, 3, 3, dtype=torch.float64)
+        for wd in windows:
+            pred = torch.randn(B, 4, len(wd), 3, 3, generator=g, dtype=torch.float64)
+            noise[:, :, wd] = noise[:, :, wd] + pred
+            counter[:, :, wd] = counter[:, :, wd] + 1
+            accumulate(acc, pred.permute(0, 2, 1, 3, 4), wd)
+        if cfg:
+            u, c = (noise / counter).chunk(2)
+            noise = u + 3.5 * (c - u)
+        got = combine(acc, inv.double(), 3.5)
+        assert torch.allclose(got, noise[0].permute(1, 0, 2, 3), rtol=1e-12, atol=1e-12), cfg
+
+
 def test_plan_units_covers_every_window_branch_once_and_balances():
     """(window, CFG branch) work units (SURVEY.md §8e): every unit is assigned exactly once, every rank derives the same
     plan, and 11 windows on 8 ranks balance better than whole windows (2 windows = 4.4 cost units on the busiest rank)."""

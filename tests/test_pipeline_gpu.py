@@ -34,6 +34,28 @@ def test_pipeline_against_reference_golden(cuda_dev):
     assert 0.0 <= out.videos.min() and out.videos.max() <= 1.0
 
 
+def test_pipeline_no_cfg_against_reference_golden(cuda_dev):
+    """pipeline_small without CFG (guidance 1.0), against the unmodified reference (tests/golden/pipeline_small_no_cfg.pt).
+    L = 20 gives two windows sharing 12 frames; without CFG the reference steps on the SUM of their predictions
+    (pipeline_pose2vid_long.py:551-559 divide by the counter only under CFG), so an averaging product fails here."""
+    gold = torch.load(os.path.join(GOLDEN, "pipeline_small_no_cfg.pt"))
+    P = gold["params"]
+    assert P["guidance"] == 1.0 and P["L"] == 20
+    pipe = build_pipeline(P, cuda_dev)
+    ref_image, poses, ref_pose = pipeline_inputs(P["size"], P["L"], P["seeds"]["inputs"])
+    trace = []
+    g = torch.manual_seed(P["seeds"]["latents"])
+    lat0 = torch.randn((1, 4, P["L"], P["size"] // 8, P["size"] // 8), generator=g, dtype=torch.float32)
+    out = pipe(ref_image, poses, ref_pose, P["size"], P["size"], P["L"], P["steps"], P["guidance"],
+               latents=lat0.to(torch.float16), callback=lambda i, t, l: trace.append(l.clone()), callback_steps=1)
+    assert out.videos.shape == (1, 3, P["L"], P["size"], P["size"])
+    e_first = rel_l2(trace[0], gold["first_step_latents"])
+    e_final = rel_l2(trace[-1], gold["final_latents"])
+    e_video = rel_l2(out.videos[:, :, [0, 7, P["L"] - 1]], gold["video_frames"])
+    print(f"no-CFG pipeline rel-L2: first step {e_first:.3e}, final latents {e_final:.3e}, video frames {e_video:.3e}")
+    assert e_first < 1e-2 and e_final < 1e-2 and e_video < 1e-2
+
+
 def test_pipeline_c1_full_width_against_reference_golden(cuda_dev):
     """BASELINE.json configs[0] (SURVEY.md 8d C1) at the REAL sizes: 512x512, L=4, 10 DDIM steps, CFG 3.5, full-width
     UNets / PoseGuider / sd-vae-ft-mse-sized VAE / ViT-L/14 CLIP with seeded weights, against the golden output of the
