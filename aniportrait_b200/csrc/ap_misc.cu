@@ -459,6 +459,28 @@ __global__ void gather_window_kernel(const __half* __restrict__ lat, const int* 
   for (int u = 1; u < Cpad / 8; ++u) o[u] = make_uint4(0u, 0u, 0u, 0u);
 }
 
+// gather_window with the UNet input scaled: out = fp16_rn(fp32(lat) * scale[0]), one rounding. The scale is read from
+// device memory so that a captured graph sees each step's value (EulerDiscreteScheduler.scale_model_input).
+__global__ void gather_window_scaled_kernel(const __half* __restrict__ lat, const int* __restrict__ idx,
+                                            const float* __restrict__ scale, __half* __restrict__ out, int dup, int F,
+                                            int HW, int Cpad) {
+  griddep_launch_dependents();   // PDL: see ap_host.h::launch_pdl
+  griddep_wait();
+  const long long total = (long long)dup * F * HW;
+  long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int px = (int)(t % HW);
+  const int f = (int)((t / HW) % F);
+  const float s = scale[0];
+  const uint2 v = *reinterpret_cast<const uint2*>(lat + ((long long)idx[f] * HW + px) * 4);
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+  const __half2 lo = __floats2half2_rn(a.x * s, a.y * s), hi = __floats2half2_rn(b.x * s, b.y * s);
+  uint4* o = reinterpret_cast<uint4*>(out + t * Cpad);
+  o[0] = make_uint4(*reinterpret_cast<const unsigned*>(&lo), *reinterpret_cast<const unsigned*>(&hi), 0u, 0u);
+  for (int u = 1; u < Cpad / 8; ++u) o[u] = make_uint4(0u, 0u, 0u, 0u);
+}
+
 // acc[b, idx[f], px, :] += pred[(b, f), px, 0..4)   (fp32 accumulation of overlapping windows)
 // A window that holds the same frame twice (dilated windows wrapping around a short clip) contributes that frame ONCE, from
 // its last occurrence — the semantics of the reference's index assignment noise_pred[:, :, c] = noise_pred[:, :, c] + pred
@@ -513,6 +535,38 @@ __global__ void cfg_ddim_step_kernel(float* __restrict__ acc, const float* __res
   const float eps = c_ex * x + c_ev * v;
   if (clip > 0.f) x0 = fminf(fmaxf(x0, -clip), clip);
   lat[t] = __float2half_rn(sqrt_ap * x0 + sqrt_bp * eps);
+}
+
+// noise = acc * inv_count ; CFG as above ; then one step of a multistep sampler (DPM-Solver(++) order 1 / 2, Euler):
+//   m = c_xx x + c_xv v   (x0, or eps for dpmsolver)      x_next = k_x x + k_0 m + k_1 m_prev
+// m_prev is the previous step's m, kept in fp32 in `hist`. hist is read only when k_1 != 0 (at the first step it holds
+// whatever the buffer held, and 0 * NaN = NaN), and overwritten with m when the next step reads it (store).
+__global__ void cfg_multistep_step_kernel(float* __restrict__ acc, const float* __restrict__ inv_count, int cfg,
+                                          float guidance, float c_xx, float c_xv, float k_x, float k_0, float k_1,
+                                          int store, float* __restrict__ hist, __half* __restrict__ lat, int L, int HW) {
+  griddep_launch_dependents();   // PDL: see ap_host.h::launch_pdl
+  griddep_wait();
+  const long long total = (long long)L * HW * 4;
+  long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int f = (int)(t / ((long long)HW * 4));
+  const float ic = inv_count[f];
+  float v;
+  if (cfg) {
+    const float u = acc[t] * ic;
+    const float c = acc[total + t] * ic;
+    v = u + guidance * (c - u);
+    acc[total + t] = 0.f;
+  } else {
+    v = acc[t] * ic;
+  }
+  acc[t] = 0.f;
+  const float x = __half2float(lat[t]);
+  const float m = c_xx * x + c_xv * v;
+  float y = k_x * x + k_0 * m;
+  if (k_1 != 0.f) y += k_1 * hist[t];
+  if (store) hist[t] = m;
+  lat[t] = __float2half_rn(y);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -696,6 +750,19 @@ extern "C" int ap_gather_window_f16(const void* latents, const int* frame_idx, v
   return AP_OK;
 }
 
+extern "C" int ap_gather_window_scaled_f16(const void* latents, const int* frame_idx, const float* scale, void* out,
+                                           int dup, int F, int HW, int Cpad, void* stream) {
+  AP_REQUIRE(latents && frame_idx && scale && out && Cpad % 8 == 0 && Cpad >= 8, "gather_window_scaled: bad arguments");
+  AP_REQUIRE(dup >= 1 && F >= 1 && HW >= 1, "gather_window_scaled: dup=%d F=%d HW=%d must be positive", dup, F, HW);
+  AP_REQUIRE((reinterpret_cast<uintptr_t>(latents) & 7) == 0 && aligned16(out),
+             "gather_window_scaled: latents must be 8-byte and out 16-byte aligned");
+  const long long total = (long long)dup * F * HW;
+  AP_LAUNCH((gather_window_scaled_kernel), (unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream,
+      (const __half*)latents, frame_idx, scale, (__half*)out, dup, F, HW, Cpad);
+  AP_CHECK_CUDA(cudaGetLastError());
+  return AP_OK;
+}
+
 extern "C" int ap_scatter_accumulate_f16(const void* pred, int ld, const int* frame_idx, float* acc, int B, int F,
                                          int L, int HW, void* stream) {
   AP_REQUIRE(pred && frame_idx && acc, "scatter_accumulate: null pointer");
@@ -732,6 +799,21 @@ extern "C" int ap_cfg_ddim_step_f16(float* acc, const float* inv_count, int cfg,
   AP_LAUNCH((cfg_ddim_step_kernel), (unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream, 
       acc, inv_count, cfg, guidance, c_xx, c_xv, c_ex, c_ev, clip_range, sqrtf(alpha_prev), sqrtf(1.f - alpha_prev),
       (__half*)latents, L, HW);
+  AP_CHECK_CUDA(cudaGetLastError());
+  return AP_OK;
+}
+
+extern "C" int ap_cfg_multistep_step_f16(float* acc, const float* inv_count, int cfg, float guidance, float c_xx,
+                                         float c_xv, float k_x, float k_0, float k_1, int store, float* hist,
+                                         void* latents, int L, int HW, void* stream) {
+  AP_REQUIRE(acc && inv_count && latents, "cfg_multistep_step: null pointer");
+  AP_REQUIRE(L >= 1 && HW >= 1, "cfg_multistep_step: L=%d HW=%d must be positive", L, HW);
+  AP_REQUIRE(hist || (k_1 == 0.f && !store), "cfg_multistep_step: k_1 != 0 or store needs the history buffer");
+  AP_REQUIRE(isfinite(guidance) && isfinite(c_xx) && isfinite(c_xv) && isfinite(k_x) && isfinite(k_0) && isfinite(k_1),
+             "cfg_multistep_step: non-finite coefficient");
+  const long long total = (long long)L * HW * 4;
+  AP_LAUNCH((cfg_multistep_step_kernel), (unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream,
+      acc, inv_count, cfg, guidance, c_xx, c_xv, k_x, k_0, k_1, store ? 1 : 0, hist, (__half*)latents, L, HW);
   AP_CHECK_CUDA(cudaGetLastError());
   return AP_OK;
 }

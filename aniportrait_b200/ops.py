@@ -652,6 +652,24 @@ def gather_window(latents: torch.Tensor, frame_idx: torch.Tensor, dup: int, cpad
     return out
 
 
+def gather_window_scaled(latents: torch.Tensor, frame_idx: torch.Tensor, scale: torch.Tensor, dup: int,
+                         cpad: int = 64) -> torch.Tensor:
+    """gather_window with the latents multiplied by scale[0] (an fp32 device scalar read by the kernel, so a captured
+    graph sees the value of every step) and rounded to fp16 once: EulerDiscreteScheduler.scale_model_input."""
+    _ensure(latents)
+    L, h, w, c = latents.shape
+    assert c == 4 and latents.dtype == torch.float16 and latents.is_contiguous() and frame_idx.dtype == torch.int32
+    assert scale.dtype == torch.float32 and scale.is_cuda and scale.numel() >= 1
+    F = frame_idx.numel()
+    out = torch.empty(dup * F, h, w, cpad, dtype=torch.float16, device=latents.device)
+    check(lib().ap_gather_window_scaled_f16(ptr(latents), _lib.ctypes.cast(_lib.c_void_p(frame_idx.data_ptr()),
+                                                                            _lib.POINTER(_lib.c_int)),
+                                            fptr(scale), ptr(out), I(dup), I(F), I(h * w), I(cpad), stream_ptr()),
+          "ap_gather_window_scaled_f16")
+    _count()
+    return out
+
+
 def scatter_accumulate(pred: torch.Tensor, frame_idx: torch.Tensor, acc: torch.Tensor):
     """pred [(B F), H, W, ld] fp16 (first 4 channels) accumulated into acc fp32 [B, L, H, W, 4] at frame_idx."""
     _ensure(pred)
@@ -683,6 +701,23 @@ def cfg_ddim_step(acc: torch.Tensor, inv_count: torch.Tensor, guidance: float, a
                                      _lib.c_float(alpha_t), _lib.c_float(alpha_prev),
                                      I(PREDICTION_TYPES[prediction_type]), _lib.c_float(clip_range), ptr(latents),
                                      I(L), I(h * w), stream_ptr()), "ap_cfg_ddim_step_f16")
+    _count()
+
+
+def cfg_multistep_step(acc: torch.Tensor, inv_count: torch.Tensor, guidance: float, coef, latents: torch.Tensor,
+                       hist: torch.Tensor):
+    """In place: one step of a multistep sampler on the CFG-combined prediction v = acc * inv_count (weights as in
+    cfg_ddim_step); acc zeroed. coef: pipelines.scheduler.MultistepCoefficients (m = c_xx x + c_xv v, latents <- k_x x +
+    k_0 m + k_1 hist, hist <- m if coef.store). hist: fp32 [L, H, W, 4], read only when k_1 != 0."""
+    _ensure(latents)
+    B, L, h, w, _ = acc.shape
+    assert latents.shape == (L, h, w, 4) and latents.dtype == torch.float16 and inv_count.dtype == torch.float32
+    assert hist.shape == (L, h, w, 4) and hist.dtype == torch.float32 and hist.is_contiguous()
+    f = _lib.c_float
+    check(lib().ap_cfg_multistep_step_f16(fptr(acc), fptr(inv_count), I(1 if B == 2 else 0), f(guidance), f(coef.c_xx),
+                                          f(coef.c_xv), f(coef.k_x), f(coef.k_0), f(coef.k_1), I(1 if coef.store else 0),
+                                          fptr(hist), ptr(latents), I(L), I(h * w), stream_ptr()),
+          "ap_cfg_multistep_step_f16")
     _count()
 
 

@@ -29,6 +29,7 @@ from ..models.clip_vision import kernels_enabled
 from ..models.mutual_self_attention import ReferenceAttentionControl
 from .sharding import plan_units, plan_windows, step_weights, windows_of_rank
 from .image_processor import VaeImageProcessor
+from .scheduler import multistep_coefficients, update_family
 
 
 class _Session:
@@ -255,6 +256,13 @@ class Pose2VideoPipeline:
         a_p = float(sch.alphas_cumprod[prev]) if prev >= 0 else float(sch.final_alpha_cumprod)
         return a_t, a_p
 
+    def _gather(self, S, idx, dup):
+        """UNet input of one call: the latents of the window's frames, times Euler's per-step input scale
+        (scale_model_input, read from S.scale_dev on the device) when the session steps with EulerDiscreteScheduler."""
+        if S.family == "euler":
+            return ops.gather_window_scaled(S.lat, idx, S.scale_dev, dup, 64)
+        return ops.gather_window(S.lat, idx, dup, 64)
+
     # -------------------------------------------------------------------------------------------- per-video stages
     # The work of one video is split into stages that only read / write the tensors of a _Session, so that each stage can
     # either run eagerly or be captured once into a CUDA graph and replayed for every later video of the same geometry.
@@ -296,7 +304,7 @@ class Pose2VideoPipeline:
 
     def _window_step(self, S, k):
         idx = S.win_idx[k]
-        x = ops.gather_window(S.lat, idx, S.dup, 64)
+        x = self._gather(S, idx, S.dup)
         pred = self.denoising_unet.forward_nhwc(x, S.dup, idx.numel(), S.t_dev, S.ehs, S.win_pose[k],
                                                 ehs_key=S.video_key)
         ops.scatter_accumulate(pred, idx, S.acc)
@@ -321,7 +329,7 @@ class Pose2VideoPipeline:
         G = S.groups[gi]
         n, nu = len(G["elems"]), G["n_uncond"]
         F = S.win_idx[G["elems"][0][0]].numel()
-        x = ops.gather_window(S.lat, G["idx_all"], 1, 64)
+        x = self._gather(S, G["idx_all"], 1)
         pred = self.denoising_unet.forward_nhwc(x, n, F, S.t_dev, G["ehs"], G["pose"], ehs_key=S.video_key,
                                                 group=(nu, n - nu))
         for e, (k, b) in enumerate(G["elems"]):
@@ -337,7 +345,7 @@ class Pose2VideoPipeline:
             return self._window_step(S, k)
         idx = S.win_idx[k]
         b = 0 if branch == "uncond" else 1
-        x = ops.gather_window(S.lat, idx, 1, 64)
+        x = self._gather(S, idx, 1)
         pred = self.denoising_unet.forward_nhwc(x, 1, idx.numel(), S.t_dev, S.ehs[b:b + 1], S.win_pose[k],
                                                 ref_branch=branch, ehs_key=S.video_key)
         ops.scatter_accumulate(pred, idx, S.acc[b:b + 1])
@@ -356,7 +364,7 @@ class Pose2VideoPipeline:
         return hash(tuple((p.data_ptr(), p._version) for m in self._nn_modules() for p in m.parameters()))
 
     def _new_session(self, clip_in, clip_is_embed, ref_image_tensor, pose_cond, L, h, w, dup, my_windows, units, static,
-                     shard):
+                     shard, family="ddim"):
         device = self.device
         S = _Session()
         # key of the per-block step-invariant caches (attn2 constant, bank K/V): one per session, never reused, so a later
@@ -376,6 +384,11 @@ class Pose2VideoPipeline:
         S.lat = torch.empty(L, h, w, 4, dtype=torch.float16, device=device)
         S.acc = torch.zeros(dup, L, h, w, 4, dtype=torch.float32, device=device)
         S.t_dev = torch.zeros(1, dtype=torch.float32, device=device)
+        # multistep samplers: the UNet input scale of the current step (Euler) and the previous step's converted model
+        # output (DPM order 2), fp32 [L, h, w, 4]; a video's first step never reads it
+        S.family = family
+        S.scale_dev = torch.ones(1, dtype=torch.float32, device=device)
+        S.hist = torch.empty(L, h, w, 4, dtype=torch.float32, device=device) if family != "ddim" else None
         S.ehs = S.ref_latents = S.win_pose = None
         S.win_idx = [torch.tensor(wd, dtype=torch.int32, device=device) for wd in my_windows]
         S.win_idx_long = [i.long() for i in S.win_idx]
@@ -511,7 +524,10 @@ class Pose2VideoPipeline:
         All stages of a video geometry are captured into CUDA graphs once (a cached _Session) and replayed for every later
         video — also in the sharded modes ("windows" / "window_branches"), where each rank captures ITS units and the two
         collectives stay eager NCCL calls between graph replays: one broadcast of the flat bank buffer per video, one fp32
-        all-reduce of the prediction accumulator per DDIM step. use_cuda_graph=False runs the same stages eagerly."""
+        all-reduce of the prediction accumulator per DDIM step. use_cuda_graph=False runs the same stages eagerly.
+        The update after each step's predictions follows the scheduler: DDIMScheduler (and any DDIM-style scheduler with
+        `alphas_cumprod`) -> ops.cfg_ddim_step; DPMSolverMultistepScheduler / EulerDiscreteScheduler -> ops.cfg_multistep_step
+        with the coefficients of scheduler.multistep_coefficients (Euler also scales the UNet input every step)."""
         device = self.device
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         ev[0].record()
@@ -528,9 +544,13 @@ class Pose2VideoPipeline:
         self.phase_detail = detail
         cfg = guidance_scale > 1.0
         dup = 2 if cfg else 1
-        pred_type, clip_range = self._scheduler_update_rule()
+        family = update_family(self.scheduler)
+        if family == "ddim":
+            pred_type, clip_range = self._scheduler_update_rule()
         self.scheduler.set_timesteps(num_inference_steps, device=device)
-        timesteps = [int(t) for t in self.scheduler.timesteps]
+        coefs = multistep_coefficients(self.scheduler) if family != "ddim" else None
+        # Euler's timesteps are fractional: the UNet's time embedding takes them as they are
+        timesteps = [float(t) if family == "euler" else int(t) for t in self.scheduler.timesteps]
         rank, world = 0, 1
         if dist_mode is not None and torch.distributed.is_available() and torch.distributed.is_initialized():
             rank, world = torch.distributed.get_rank(), torch.distributed.get_world_size()
@@ -558,7 +578,7 @@ class Pose2VideoPipeline:
             # the last entry: clip_vision.enable_kernels rebinds the encoder's forward without touching its parameters, so
             # the fingerprint does not see it; a session captured on the other CLIP path must not be replayed
             key = (L, h, w, dup, tuple(tuple(wd) for wd in my_windows), tuple(units), shard, rank, world,
-                   self.group_units if shard else 0, clip_is_embed,
+                   self.group_units if shard else 0, clip_is_embed, family,
                    tuple(clip_in.shape), tuple(ref_image_tensor.shape), tuple(pose_cond.shape),
                    self._weights_fingerprint(), kernels_enabled(self.image_encoder))
             S = self._sessions.get(key)
@@ -566,7 +586,7 @@ class Pose2VideoPipeline:
                 while len(self._sessions) >= self.max_sessions:     # each session pins ~10 GB of activations
                     self._sessions.pop(next(iter(self._sessions)))
                 S = self._new_session(clip_in, clip_is_embed, ref_image_tensor, pose_cond, L, h, w, dup, my_windows, units,
-                                      True, shard)
+                                      True, shard, family)
                 S.lat.copy_(latents[0].permute(1, 2, 3, 0))
                 self._build_static_session(S, mark)
                 self._sessions[key] = S
@@ -580,7 +600,7 @@ class Pose2VideoPipeline:
             mark("prologue_replay_ms")
         else:
             S = self._new_session(clip_in, clip_is_embed, ref_image_tensor, pose_cond, L, h, w, dup, my_windows, units,
-                                  False, shard)
+                                  False, shard, family)
             S.lat.copy_(latents[0].permute(1, 2, 3, 0))
             self._stage_embed(S)
             mark("embed_ms")
@@ -597,6 +617,8 @@ class Pose2VideoPipeline:
         with self.progress_bar(total=num_inference_steps) as progress_bar:
             for i, t in enumerate(timesteps):
                 S.t_dev.fill_(float(t))
+                if coefs is not None:
+                    S.scale_dev.fill_(coefs[i].scale)
                 if static:
                     for g, n in zip(S.g_units, S.n_units):
                         g.replay()
@@ -610,8 +632,11 @@ class Pose2VideoPipeline:
                     torch.distributed.all_reduce(acc)
                     e1.record()
                     self._comm_events.append(("all_reduce_ms", e0, e1))
-                a_t, a_p = self._alpha_pair(t)
-                ops.cfg_ddim_step(acc, inv_count, float(guidance_scale), a_t, a_p, lat, pred_type, clip_range)
+                if coefs is None:
+                    a_t, a_p = self._alpha_pair(t)
+                    ops.cfg_ddim_step(acc, inv_count, float(guidance_scale), a_t, a_p, lat, pred_type, clip_range)
+                else:
+                    ops.cfg_multistep_step(acc, inv_count, float(guidance_scale), coefs[i], lat, S.hist)
                 progress_bar.update()
                 if callback is not None and i % callback_steps == 0:
                     callback(i, t, lat.permute(3, 0, 1, 2).unsqueeze(0))
@@ -698,6 +723,10 @@ class Pose2VideoPipeline:
             clip_src = ref_image.resize((224, 224)) if clip_resize else ref_image
             clip_pixels = self.clip_image_processor.preprocess(clip_src, return_tensors="pt").pixel_values
         embed_dtype = self.image_encoder.dtype if isinstance(self.image_encoder, torch.nn.Module) else torch.float16
+        update_family(self.scheduler)      # schedulers the fused updates cannot reproduce raise before any work
+        # as the reference (:373, :409): the timesteps first, then the initial noise times init_noise_sigma, which for
+        # EulerDiscreteScheduler depends on them (leading spacing)
+        self.scheduler.set_timesteps(num_inference_steps, device=device)
         latents = self.prepare_latents(num_images_per_prompt, self.denoising_unet.in_channels, width, height,
                                        video_length, embed_dtype, device, generator, latents)
         ref_image_tensor = self.ref_image_processor.preprocess(ref_image, height=height, width=width)

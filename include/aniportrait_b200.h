@@ -332,6 +332,22 @@ int ap_cfg_ddim_step_f16(float* acc, const float* inv_count, int cfg, float guid
                          int prediction_type, float clip_range, void* latents, int L, int HW, void* stream);
 
 /*
+ * Multistep samplers (diffusers 0.24 DPMSolverMultistepScheduler of order 1 / 2 and EulerDiscreteScheduler without churn,
+ * pipelines/scheduler.py::multistep_coefficients). Same layouts as above.
+ * ap_cfg_multistep_step_f16: per-frame weighting + classifier-free guidance as ap_cfg_ddim_step_f16, then
+ *   m = c_xx x + c_xv v,   latents <- fp16_rn(k_x x + k_0 m + k_1 hist),   hist <- m if store (fp32 [L, HW, 4]);
+ * `acc` is zeroed. hist is read only when k_1 != 0 (its contents before the first step are never read) and may be NULL
+ * when k_1 == 0 and store == 0. Null pointers, L or HW < 1 and non-finite coefficients return AP_ERR_INVALID, no launch.
+ * ap_gather_window_scaled_f16: ap_gather_window_f16 with the 4 latent channels multiplied by scale[0] (device memory,
+ * so captured graphs read each step's value) and rounded to fp16 once; same alignment and size rules.
+ */
+int ap_cfg_multistep_step_f16(float* acc, const float* inv_count, int cfg, float guidance, float c_xx, float c_xv,
+                              float k_x, float k_0, float k_1, int store, float* hist, void* latents, int L, int HW,
+                              void* stream);
+int ap_gather_window_scaled_f16(const void* latents, const int* frame_idx, const float* scale, void* out, int dup, int F,
+                                int HW, int Cpad, void* stream);
+
+/*
  * Decoded video -> packed 8-bit RGB frames on the device (reference src/utils/util.py:87-104 save_videos_grid does
  * `(x * 255).numpy().astype(np.uint8)`, after `(x + 1) / 2` if rescale, on the fp32 host copy that
  * pipeline_pose2vid_long.py:123-125 makes: 4 bytes per sample over PCIe instead of 1). video: fp16 [B, 3, F, H, W] addressed
